@@ -240,16 +240,17 @@ struct abb_graph {
     DevBuf d_roots, d_root_off, d_targets, d_qstart, d_qcount, d_qmaxd, d_qflags, d_qestart, d_qecount, d_qhist;
     DevBuf d_nodes, d_parent, d_depth, d_edges, d_totals;
     int64_t hint_nodes = 0, hint_edges = 0, hint_nq = 0, hint_last_nodes = 0;
-    // graph-constant server fan-out table (built on first use)
-    DevBuf srv_cred, srv_tool;
+    // graph-constant server tables (built on first use): fan-out, and the principal rows each server contributes to a template
+    DevBuf srv_cred, srv_tool, srv_roff, srv_row, srv_rel;
     bool srv_table_ready = false;
     // paths staging
     DevBuf p_findings, p_counts, p_off, p_hops, p_rels, p_ncred, p_ntool, p_scan_tmp;
     // exposure-path pipeline workspace (links, templates)
-    DevBuf pl_cnt, pl_off, pl_vs, pl_rel, pl_rows, pl_roff, pl_toff, pl_need, pl_ulist, pl_nu, pt_cnt, pt_off, pt_off_node, pt_cnt_node, pt_row, pt_rel;
+    DevBuf pl_cnt, pl_off, pl_vs, pl_rel, pl_f, pl_rows, pl_roff, pl_toff, pl_need, pl_ulist, pl_nu, pt_cnt, pt_off, pt_off_node, pt_cnt_node, pt_row, pt_rel;
     PathsArgs paths_args{};
     bool paths_args_valid = false;
     int64_t paths_n_links = 0, paths_n_template_rows = 0;
+    int replicate_grid = 0, rank_keys_grid = 0;   // grids of the row-parallel kernels (row_grid)
     int64_t hint_rows = 0;
     // owned graph arrays
     std::vector<void *> owned_ptrs;
@@ -1307,20 +1308,6 @@ extern "C" int abb_walk_host(abb_graph *g, const abb_walk_spec *spec, const int3
 }
 
 // ------------------------------------------------------------------ exposure-path rows
-static int ensure_server_table(abb_graph *g, cudaStream_t st) {
-    if (g->srv_table_ready) return ABB_OK;
-    const size_t n = static_cast<size_t>(g->v.n) + 1;
-    if (int rc = g->srv_cred.ensure(n * 4)) return rc;
-    if (int rc = g->srv_tool.ensure(n * 4)) return rc;
-    const int64_t blocks = std::min<int64_t>((g->v.n + 255) / 256, static_cast<int64_t>(g->sm_count) * 16);
-    server_table_kernel<<<static_cast<unsigned>(std::max<int64_t>(1, blocks)), 256, 0, st>>>(g->v, g->srv_cred.as<int32_t>(), g->srv_tool.as<int32_t>());
-    g_launches++;
-    CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaStreamSynchronize(st));   // one-time: later launches may come on other streams
-    g->srv_table_ready = true;
-    return ABB_OK;
-}
-
 static int scan_i64(abb_graph *g, const int64_t *in, int64_t *out, int64_t n, cudaStream_t st) {
     size_t tmp = 0;
     CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tmp, in, out, static_cast<int>(n), st));
@@ -1330,8 +1317,50 @@ static int scan_i64(abb_graph *g, const int64_t *in, int64_t *out, int64_t n, cu
     return ABB_OK;
 }
 
+static int ensure_server_table(abb_graph *g, cudaStream_t st) {
+    if (g->srv_table_ready) return ABB_OK;
+    const size_t n = static_cast<size_t>(g->v.n) + 1;
+    if (int rc = g->srv_cred.ensure(n * 4)) return rc;
+    if (int rc = g->srv_tool.ensure(n * 4)) return rc;
+    const int64_t blocks = std::min<int64_t>((g->v.n + 255) / 256, static_cast<int64_t>(g->sm_count) * 16);
+    const unsigned grid = static_cast<unsigned>(std::max<int64_t>(1, blocks));
+    server_table_kernel<<<grid, 256, 0, st>>>(g->v, g->srv_cred.as<int32_t>(), g->srv_tool.as<int32_t>());
+    g_launches++;
+    // principal rows of every server (paths.cuh server_rows_kernel): count, scan in place, fill
+    if (int rc = g->srv_roff.ensure(n * 8)) return rc;
+    int64_t *roff = g->srv_roff.as<int64_t>();
+    CUDA_TRY(cudaMemsetAsync(roff, 0, n * 8, st));
+    server_rows_kernel<false><<<grid, 256, 0, st>>>(g->v, g->srv_cred.as<int32_t>(), g->srv_tool.as<int32_t>(), roff, nullptr, nullptr);
+    g_launches++;
+    if (int rc = scan_i64(g, roff, roff, static_cast<int64_t>(n), st)) return rc;
+    int64_t total = 0;
+    CUDA_TRY(cudaMemcpyAsync(&total, roff + g->v.n, 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (int rc = g->srv_row.ensure(static_cast<size_t>(total + 1) * 16)) return rc;
+    if (int rc = g->srv_rel.ensure(static_cast<size_t>(total) + 16)) return rc;
+    server_rows_kernel<true><<<grid, 256, 0, st>>>(g->v, g->srv_cred.as<int32_t>(), g->srv_tool.as<int32_t>(), roff, g->srv_row.as<int4>(), g->srv_rel.as<int8_t>());
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaStreamSynchronize(st));   // one-time: later launches may come on other streams
+    g->srv_table_ready = true;
+    return ABB_OK;
+}
+
 static unsigned warp_grid(const abb_graph *g, int64_t warps) {
     return static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>((warps + 7) / 8, static_cast<int64_t>(g->sm_count) * 8)));
+}
+
+// for_each_row gives each block an equal contiguous run of row tiles, so the grid is a whole number of waves of resident blocks
+// (a partial last wave would add a block's whole run to the time).  Four waves rather than one, so that blocks still start
+// promptly when another stream's kernels hold part of the GPU.
+template <class K>
+static unsigned row_grid(const abb_graph *g, K kernel, int &cached) {
+    if (!cached) {
+        int per_sm = 0;
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, ROW_THREADS, 0);
+        cached = 4 * g->sm_count * std::max(1, per_sm);
+    }
+    return static_cast<unsigned>(cached);
 }
 
 // Count pass of the exposure-path pipeline (paths.cuh): links -> unique vulnerable sources -> templates -> per-finding
@@ -1345,6 +1374,7 @@ static int enqueue_paths_count(abb_graph *g, const abb_paths_io *io, cudaStream_
     const int64_t nf = io->n_findings, n = g->v.n;
     PathsArgs A{};
     A.g = g->v; A.io = *io; A.srv_cred = g->srv_cred.as<int32_t>(); A.srv_tool = g->srv_tool.as<int32_t>();
+    A.srv_roff = g->srv_roff.as<int64_t>(); A.srv_row = g->srv_row.as<int4>(); A.srv_rel = g->srv_rel.as<int8_t>();
     int rc = ABB_OK;
 #define ENS(buf, bytes) if (!rc) rc = g->buf.ensure(static_cast<size_t>(bytes))
     ENS(pl_cnt, (nf + 2) * 8); ENS(pl_off, (nf + 2) * 8); ENS(pl_need, n + 16); ENS(pl_ulist, (n + 2) * 4); ENS(pl_nu, 16);
@@ -1355,18 +1385,18 @@ static int enqueue_paths_count(abb_graph *g, const abb_paths_io *io, cudaStream_
     A.t_off_node = g->pt_off_node.as<int64_t>(); A.t_cnt_node = g->pt_cnt_node.as<int32_t>();
     A.n_links = reinterpret_cast<const unsigned long long *>(A.link_off + nf);
     CUDA_TRY(cudaMemsetAsync(A.link_cnt, 0, static_cast<size_t>(nf + 2) * 8, st));
-    if (nf) { links_kernel<false><<<warp_grid(g, nf), 256, 0, st>>>(A); g_launches++; }
+    if (nf) { links_kernel<false><<<warp_grid(g, (nf + 31) / 32), 256, 0, st>>>(A); g_launches++; }
     if ((rc = scan_i64(g, A.link_cnt, A.link_off, nf + 1, st))) return rc;
     int64_t NL = 0;
     CUDA_TRY(cudaMemcpyAsync(&NL, A.link_off + nf, 8, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     const int64_t nu_max = std::min<int64_t>(NL, n);
-    ENS(pl_vs, (NL + 2) * 4); ENS(pl_rel, NL + 16); ENS(pl_rows, (NL + 2) * 8); ENS(pl_roff, (NL + 2) * 8); ENS(pl_toff, (NL + 2) * 8); ENS(pt_cnt, (nu_max + 2) * 8); ENS(pt_off, (nu_max + 2) * 8);
+    ENS(pl_vs, (NL + 2) * 4); ENS(pl_rel, NL + 16); ENS(pl_f, (NL + 2) * 4); ENS(pl_rows, (NL + 2) * 8); ENS(pl_roff, (NL + 2) * 8); ENS(pl_toff, (NL + 2) * 8); ENS(pt_cnt, (nu_max + 2) * 8); ENS(pt_off, (nu_max + 2) * 8);
     if (rc) return rc;
-    A.link_vs = g->pl_vs.as<int32_t>(); A.link_rel = g->pl_rel.as<int8_t>(); A.link_rows = g->pl_rows.as<int64_t>(); A.link_roff = g->pl_roff.as<int64_t>(); A.link_toff = g->pl_toff.as<int64_t>();
+    A.link_vs = g->pl_vs.as<int32_t>(); A.link_rel = g->pl_rel.as<int8_t>(); A.link_f = g->pl_f.as<int32_t>(); A.link_rows = g->pl_rows.as<int64_t>(); A.link_roff = g->pl_roff.as<int64_t>(); A.link_toff = g->pl_toff.as<int64_t>();
     A.t_cnt = g->pt_cnt.as<int64_t>(); A.t_off = g->pt_off.as<int64_t>();
     CUDA_TRY(cudaMemsetAsync(A.need, 0, static_cast<size_t>(n) + 16, st));
-    if (nf) { links_kernel<true><<<warp_grid(g, nf), 256, 0, st>>>(A); g_launches++; }
+    if (nf) { links_kernel<true><<<warp_grid(g, (nf + 31) / 32), 256, 0, st>>>(A); g_launches++; }
     // unique vulnerable sources, node order
     {
         cub::CountingInputIterator<int32_t> iota(0);
@@ -1377,7 +1407,7 @@ static int enqueue_paths_count(abb_graph *g, const abb_paths_io *io, cudaStream_
         g_launches++;
     }
     CUDA_TRY(cudaMemsetAsync(A.t_cnt, 0, static_cast<size_t>(nu_max + 2) * 8, st));
-    if (nu_max) { template_kernel<false><<<warp_grid(g, nu_max), 256, 0, st>>>(A); g_launches++; }
+    if (nu_max) { template_kernel<false><<<warp_grid(g, (nu_max + 31) / 32), 256, 0, st>>>(A); g_launches++; }
     if ((rc = scan_i64(g, A.t_cnt, A.t_off, nu_max + 1, st))) return rc;
     int64_t TR = 0;
     CUDA_TRY(cudaMemcpyAsync(&TR, A.t_off + nu_max, 8, cudaMemcpyDeviceToHost, st));
@@ -1386,7 +1416,7 @@ static int enqueue_paths_count(abb_graph *g, const abb_paths_io *io, cudaStream_
     if (rc) return rc;
 #undef ENS
     A.t_row = g->pt_row.as<int4>(); A.t_rel = g->pt_rel.as<int8_t>();
-    if (nu_max) { template_kernel<true><<<warp_grid(g, nu_max), 256, 0, st>>>(A); g_launches++; }
+    if (nu_max) { template_kernel<true><<<warp_grid(g, (nu_max + 31) / 32), 256, 0, st>>>(A); g_launches++; }
     CUDA_TRY(cudaMemsetAsync(A.link_rows, 0, static_cast<size_t>(NL + 2) * 8, st));
     if (NL) { link_rows_kernel<<<static_cast<unsigned>((NL + 255) / 256), 256, 0, st>>>(A); g_launches++; }
     if ((rc = scan_i64(g, A.link_rows, A.link_roff, NL + 1, st))) return rc;
@@ -1406,7 +1436,7 @@ static int enqueue_paths_fill(abb_graph *g, const abb_paths_io *io, cudaStream_t
     if ((reinterpret_cast<uintptr_t>(io->hops) & 15) != 0 || (reinterpret_cast<uintptr_t>(io->rels) & 3) != 0) return fail(ABB_ERR_ARG, "io.hops must be 16-byte and io.rels 4-byte aligned");
     PathsArgs A = g->paths_args;
     A.io = *io;
-    replicate_kernel<<<warp_grid(g, (io->n_findings + 31) / 32), 256, 0, st>>>(A);
+    replicate_kernel<<<row_grid(g, replicate_kernel, g->replicate_grid), ROW_THREADS, 0, st>>>(A);
     g_launches++;
     CUDA_TRY(cudaGetLastError());
     return ABB_OK;
@@ -1634,7 +1664,7 @@ extern "C" int abb_paths_rank_host(abb_graph *g, const int32_t *findings, int64_
     if (rc) { delete r; return rc; }
     PathsArgs A = g->paths_args;
     RankArgs RA{d_base.as<int32_t>(), d_tab.as<uint32_t>(), d_ncu.as<int32_t>(), d_ntu.as<int32_t>(), k1.as<unsigned long long>(), v1.as<uint32_t>()};
-    rank_keys_kernel<<<warp_grid(g, (nf + 31) / 32), 256, 0, st>>>(A, RA); g_launches++;
+    rank_keys_kernel<<<row_grid(g, rank_keys_kernel, g->rank_keys_grid), ROW_THREADS, 0, st>>>(A, RA); g_launches++;
     size_t tb = 0;
     cudaError_t ce = cub::DeviceRadixSort::SortPairs(nullptr, tb, k1.as<unsigned long long>(), k2.as<unsigned long long>(), v1.as<uint32_t>(), v2.as<uint32_t>(),
                                                      static_cast<int>(R), 0, 64, st);

@@ -11,14 +11,18 @@
 //               ncred / ntool = # EXPOSES_CRED / PROVIDES_TOOL out-edges whose target has a node record
 //   row (agent, server, vs, f) + first relationship per hop pair.
 //
-// One warp per finding, two passes over the same code (count, then fill at the
-// scanned offsets) so rows land in the reference's emission order.  Inside a
-// finding the reverse row of vs is consumed 32 entries at a time and each lane
-// owns one candidate server (its own short reverse row is walked lane-serially),
-// so a popular package with hundreds of dependent servers is handled 32 servers
-// per step instead of one.  "Originals only" = entries without
-// ABB_META_REVERSED_COPY: the reference builds its incoming/outgoing maps from
-// graph.edges, which never holds the reversed copies of bidirectional edges (:698-702).
+// The rows are factorised: a finding's LINKS (one per vulnerable source vs) and,
+// per distinct vs, a TEMPLATE (its (agent, server) rows), which every finding
+// attached to vs shares.  The principals of a server depend only on the graph, so
+// they sit in a graph-constant server row table built once per graph
+// (server_rows_kernel); a template is the concatenation of its servers' table
+// rows.  Links and templates are built per call with one thread per finding /
+// vulnerable source in two passes (count, then fill at the scanned offsets) so
+// rows land in the reference's emission order; reverse rows longer than LONG_ROW
+// are handed to the whole warp.  The flat rows are then written row-parallel
+// (for_each_row).  "Originals only" = entries without ABB_META_REVERSED_COPY: the
+// reference builds its incoming/outgoing maps from graph.edges, which never holds
+// the reversed copies of bidirectional edges (:698-702).
 //
 // Pair relationships: by_pair.setdefault((a,b)) keeps the first edge between a
 // and b.  Entries of adjacency[a] with neighbour b and entries of
@@ -33,18 +37,23 @@ namespace abb {
 
 constexpr int REL_USES = 1, REL_DEPENDS_ON = 2, REL_PROVIDES_TOOL = 3, REL_EXPOSES_CRED = 4, REL_VULNERABLE_TO = 9;
 constexpr int ET_AGENT = 0, ET_SERVER = 1, ET_VULN = 8, ET_MISCONF = 9, ET_USER = 13, ET_SERVICE_ACCOUNT = 17;
-constexpr uint32_t LONG_ROW = 64;   // reverse rows of a server longer than this are handled by the whole warp
+constexpr uint32_t LONG_ROW = 64;   // reverse rows longer than this are handled by the whole warp
 
 struct PathsArgs {
     GraphView g;
     abb_paths_io io;
     const int32_t *srv_cred;    // [n_nodes] EXPOSES_CRED fan-out of server nodes (graph-constant table)
     const int32_t *srv_tool;    // [n_nodes] PROVIDES_TOOL fan-out
+    // graph-constant server row table: the principal rows every server contributes to a template
+    const int64_t *srv_roff;    // [n_nodes+1] first table row of each node (only servers own rows, at least one each)
+    const int4 *srv_row;        // [n_server_rows] agent, server, ncred, ntool
+    const int8_t *srv_rel;      // [n_server_rows] relationship of the pair (agent, server)
     // links: one per (finding, vulnerable source) in emission order
     int64_t *link_cnt;          // [n_findings+1] links per finding (count pass), then scanned into link_off
     int64_t *link_off;          // [n_findings+1]
     int32_t *link_vs;           // [n_links]
     int8_t *link_rel;           // [n_links] relationship of the pair (vs, finding)
+    int32_t *link_f;            // [n_links] finding index (position in io.findings) of the link
     int64_t *link_rows;         // [n_links+1] rows per link, scanned into link_roff
     int64_t *link_toff;         // [n_links] template offset of the link's vulnerable source
     int64_t *link_roff;         // [n_links+1]
@@ -134,99 +143,134 @@ __device__ __forceinline__ bool next_agent_warp(const GraphView &g, int32_t s, i
     return true;
 }
 
-// one template row: (agent, server) and the relationships of the pairs (agent,server), (server,vs)
-__device__ __forceinline__ void write_row(const PathsArgs &A, int64_t row, int32_t agent, int32_t srv, int32_t, int32_t, int rel_as, int rel_sv, int) {
-    A.t_row[row] = make_int4(agent, srv, __ldg(A.srv_cred + srv), __ldg(A.srv_tool + srv));
-    A.t_rel[row * 2] = static_cast<int8_t>(rel_as); A.t_rel[row * 2 + 1] = static_cast<int8_t>(rel_sv);
-}
-
-// Rows of up to 32 candidate servers (lane i owns server s, -1 = none) of one (finding, vulnerable source).
-// Returns the number of rows; rows are laid out in lane order from row0.
+// ---- graph-constant server row table: for every server, its principals in ascending id-string rank with the relationship of
+// the pair (agent, server), or the server itself (with the relationship of the pair (server, server)) when no principal uses it
+// (:737-738).  Lane u owns node u; a server with a long reverse row is handed to the whole warp.  COUNT writes each server's
+// row count to srv_roff[u] (scanned in place afterwards), FILL writes the rows from srv_roff[u].
 template <bool FILL>
-__device__ int64_t server_chunk(const PathsArgs &A, int64_t row0, int32_t s, int rel_sv, int32_t vs, int32_t f, int rel_vf, int lane) {
-    const GraphView &g = A.g;
-    const bool have = s >= 0;
-    const uint32_t len = have ? (__ldg(g.roff + s + 1) - __ldg(g.roff + s)) : 0;
-    const bool is_long = have && len > LONG_ROW;
-    int cnt = 0;
-    if (have && !is_long) {
-        int32_t last = -1, a; int r;
-        while (next_agent_serial(g, s, last, a, r)) cnt++;
-        if (cnt == 0) cnt = 1;                      // no agent uses the server: the path starts at the server itself (:737-738)
-    }
-    unsigned lm = __ballot_sync(FULL, is_long);
-    for (unsigned rem = lm; rem; rem &= rem - 1) {
-        const int src = __ffs(rem) - 1;
-        const int32_t ls = __shfl_sync(FULL, s, src);
-        int32_t last = -1, a; int r; int c = 0;
-        while (next_agent_warp(g, ls, last, a, r, lane)) c++;
-        if (c == 0) c = 1;
-        if (lane == src) cnt = c;
-    }
-    int inc = cnt;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(FULL, inc, o); if (lane >= o) inc += v; }
-    const int total = __shfl_sync(FULL, inc, 31);
-    if (FILL) {
-        const int64_t my0 = row0 + (inc - cnt);
-        if (have && !is_long) {
+__global__ void __launch_bounds__(256) server_rows_kernel(const GraphView g, const int32_t *srv_cred, const int32_t *srv_tool, int64_t *srv_roff, int4 *srv_row,
+                                                          int8_t *srv_rel) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warp = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+    const int64_t nwarps = (static_cast<int64_t>(gridDim.x) * blockDim.x) >> 5;
+    auto put = [&](int64_t k, int32_t a, int32_t s, int rel) {
+        srv_row[k] = make_int4(a, s, __ldg(srv_cred + s), __ldg(srv_tool + s));
+        srv_rel[k] = static_cast<int8_t>(rel);
+    };
+    for (int64_t base = warp * 32; base < g.n; base += nwarps * 32) {
+        const int64_t u = base + lane;
+        const int32_t s = (u < g.n && __ldg(g.ntype + u) == ET_SERVER) ? static_cast<int32_t>(u) : -1;
+        const bool is_long = s >= 0 && __ldg(g.roff + s + 1) - __ldg(g.roff + s) > LONG_ROW;
+        const int64_t row0 = (FILL && s >= 0) ? srv_roff[s] : 0;
+        if (s >= 0 && !is_long) {
             int32_t last = -1, a; int r; int k = 0;
-            while (next_agent_serial(g, s, last, a, r)) write_row(A, my0 + k++, a, s, vs, f, r, rel_sv, rel_vf);
-            if (k == 0) write_row(A, my0, s, s, vs, f, first_rel_rev(g, s, s), rel_sv, rel_vf);
+            while (next_agent_serial(g, s, last, a, r)) { if (FILL) put(row0 + k, a, s, r); k++; }
+            if (k == 0) { if (FILL) put(row0, s, s, first_rel_rev(g, s, s)); k = 1; }
+            if (!FILL) srv_roff[s] = k;
         }
-        for (unsigned rem = lm; rem; rem &= rem - 1) {
+        for (unsigned rem = __ballot_sync(FULL, is_long); rem; rem &= rem - 1) {
             const int src = __ffs(rem) - 1;
             const int32_t ls = __shfl_sync(FULL, s, src);
-            const int lrel = __shfl_sync(FULL, rel_sv, src);
-            const int64_t l0 = __shfl_sync(FULL, my0, src);
+            const int64_t l0 = __shfl_sync(FULL, row0, src);
             int32_t last = -1, a; int r; int k = 0;
-            while (next_agent_warp(g, ls, last, a, r, lane)) { if (lane == 0) write_row(A, l0 + k, a, ls, vs, f, r, lrel, rel_vf); k++; }
-            if (k == 0 && lane == 0) write_row(A, l0, ls, ls, vs, f, first_rel_rev(g, ls, ls), lrel, rel_vf);
+            while (next_agent_warp(g, ls, last, a, r, lane)) { if (FILL && lane == 0) put(l0 + k, a, ls, r); k++; }
+            if (k == 0) { if (FILL && lane == 0) put(l0, ls, ls, first_rel_rev(g, ls, ls)); k = 1; }
+            if (!FILL && lane == 0) srv_roff[ls] = k;
         }
     }
-    return total;
 }
 
-// ---- pass A: links of every finding (VULNERABLE_TO originals whose source has a node record), in row order
+// ---- pass A: links of every finding (VULNERABLE_TO originals whose source has a node record), in row order.
+// The source behind reverse-row entry k of a finding, or -1; rvf = relationship of the pair (vs, finding), -3 = not the first
+// entry of the pair (looked up in the fill pass).
+__device__ __forceinline__ int32_t link_source(const GraphView &g, uint32_t k, int &rvf) {
+    const uint32_t m = __ldg(g.rmeta + k);
+    if ((m & ABB_META_REVERSED_COPY) || (m & ABB_META_REL_MASK) != REL_VULNERABLE_TO) return -1;
+    const int32_t v = __ldg(g.rnbr + k);
+    if (__ldg(g.ntype + v) == ABB_NODE_GHOST) return -1;
+    rvf = (m & ABB_META_FIRST_PAIR) ? REL_VULNERABLE_TO : -3;
+    return v;
+}
+
+__device__ __forceinline__ void put_link(const PathsArgs &A, int64_t o, int32_t vs, int32_t f, int rvf, int64_t fi) {
+    if (rvf == -3) rvf = first_rel_rev(A.g, vs, f);
+    A.link_vs[o] = vs; A.link_rel[o] = static_cast<int8_t>(rvf); A.link_f[o] = static_cast<int32_t>(fi);
+    A.need[vs] = 1;
+}
+
+// one thread per finding; a finding with a long reverse row is handed to the whole warp
 template <bool FILL>
 __global__ void __launch_bounds__(256) links_kernel(const PathsArgs A) {
     const GraphView &g = A.g;
     const int lane = threadIdx.x & 31;
     const int64_t warp = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = (static_cast<int64_t>(gridDim.x) * blockDim.x) >> 5;
-    for (int64_t fi = warp; fi < A.io.n_findings; fi += nwarps) {
-        const int32_t f = __ldg(A.io.findings + fi);
+    const int64_t nf = A.io.n_findings;
+    for (int64_t base = warp * 32; base < nf; base += nwarps * 32) {
+        const int64_t fi = base + lane;
+        int32_t f = -1; uint32_t s0 = 0, e0 = 0;
+        if (fi < nf) {
+            f = __ldg(A.io.findings + fi);
+            bool ok = f >= 0 && f < g.n;
+            if (ok) { const uint8_t ft = __ldg(g.ntype + f); ok = ft == ET_VULN || ft == ET_MISCONF; }
+            if (ok) { s0 = __ldg(g.roff + f); e0 = __ldg(g.roff + f + 1); }
+        }
+        const bool is_long = e0 - s0 > LONG_ROW;
+        const int64_t o0 = (FILL && fi < nf) ? A.link_off[fi] : 0;
         int64_t n = 0;
-        const int64_t base = FILL ? A.link_off[fi] : 0;
-        bool ok = f >= 0 && f < g.n;
-        if (ok) { const uint8_t ft = __ldg(g.ntype + f); ok = ft == ET_VULN || ft == ET_MISCONF; }
-        if (ok) {
-            const uint32_t s0 = __ldg(g.roff + f), e0 = __ldg(g.roff + f + 1);
-            for (uint32_t p = s0; p < e0; p += 32) {
-                const uint32_t k = p + lane;
-                int32_t vs = -1; int rvf = -1;
-                if (k < e0) {
-                    const uint32_t m = __ldg(g.rmeta + k);
-                    if (!(m & ABB_META_REVERSED_COPY) && (m & ABB_META_REL_MASK) == REL_VULNERABLE_TO) {
-                        const int32_t v = __ldg(g.rnbr + k);
-                        if (__ldg(g.ntype + v) != ABB_NODE_GHOST) { vs = v; rvf = (m & ABB_META_FIRST_PAIR) ? REL_VULNERABLE_TO : -3; }
-                    }
-                }
-                const unsigned vm = __ballot_sync(FULL, vs >= 0);
-                if (FILL && vs >= 0) {
-                    if (rvf == -3) rvf = first_rel_rev(g, vs, f);
-                    const int64_t o = base + n + __popc(vm & lanemask_lt(lane));
-                    A.link_vs[o] = vs; A.link_rel[o] = static_cast<int8_t>(rvf);
-                    A.need[vs] = 1;
-                }
-                n += __popc(vm);
+        if (!is_long) {
+            for (uint32_t p = s0; p < e0; p++) {
+                int rvf;
+                const int32_t vs = link_source(g, p, rvf);
+                if (vs < 0) continue;
+                if (FILL) put_link(A, o0 + n, vs, f, rvf, fi);
+                n++;
             }
         }
-        if (!FILL && lane == 0) A.link_cnt[fi] = n;
+        for (unsigned rem = __ballot_sync(FULL, is_long); rem; rem &= rem - 1) {
+            const int src = __ffs(rem) - 1;
+            const int32_t lf = __shfl_sync(FULL, f, src);
+            const uint32_t ls0 = __shfl_sync(FULL, s0, src), le0 = __shfl_sync(FULL, e0, src);
+            const int64_t lo0 = __shfl_sync(FULL, o0, src), lfi = base + src;
+            int64_t ln = 0;
+            for (uint32_t p = ls0; p < le0; p += 32) {
+                const uint32_t k = p + lane;
+                int rvf = -1;
+                const int32_t vs = k < le0 ? link_source(g, k, rvf) : -1;
+                const unsigned vm = __ballot_sync(FULL, vs >= 0);
+                if (FILL && vs >= 0) put_link(A, lo0 + ln + __popc(vm & lanemask_lt(lane)), vs, lf, rvf, lfi);
+                ln += __popc(vm);
+            }
+            if (lane == src) n = ln;
+        }
+        if (!FILL && fi < nf) A.link_cnt[fi] = n;
     }
 }
 
-// ---- pass B: the template of each referenced vulnerable source (count, then fill)
+// ---- pass B: the template of each referenced vulnerable source (count, then fill): the server table's rows of vs itself when
+// it is a server, else of every server that DEPENDS_ON it, in reverse-row order.
+// The server behind reverse-row entry k of a non-server vulnerable source, or -1; rsv as rvf above.
+__device__ __forceinline__ int32_t dependent_server(const GraphView &g, uint32_t k, int &rsv) {
+    const uint32_t m = __ldg(g.rmeta + k);
+    if ((m & ABB_META_REVERSED_COPY) || (m & ABB_META_REL_MASK) != REL_DEPENDS_ON) return -1;
+    const int32_t v = __ldg(g.rnbr + k);
+    if (__ldg(g.ntype + v) != ET_SERVER) return -1;
+    rsv = (m & ABB_META_FIRST_PAIR) ? REL_DEPENDS_ON : -3;
+    return v;
+}
+
+__device__ __forceinline__ int64_t server_rows(const PathsArgs &A, int32_t s) { return __ldg(A.srv_roff + s + 1) - __ldg(A.srv_roff + s); }
+
+// server s's table rows into the template from `row`; the template's relationships are the pairs (agent, server), (server, vs)
+__device__ __forceinline__ void copy_server_rows(const PathsArgs &A, int64_t row, int32_t s, int32_t vs, int rsv) {
+    if (rsv == -3) rsv = first_rel_rev(A.g, s, vs);
+    for (int64_t k = __ldg(A.srv_roff + s), e = __ldg(A.srv_roff + s + 1); k < e; k++, row++) {
+        A.t_row[row] = __ldg(A.srv_row + k);
+        reinterpret_cast<uint16_t *>(A.t_rel)[row] = static_cast<uint16_t>(static_cast<uint8_t>(__ldg(A.srv_rel + k)) | ((rsv & 0xFF) << 8));
+    }
+}
+
+// one thread per vulnerable source; one with a long reverse row is handed to the whole warp
 template <bool FILL>
 __global__ void __launch_bounds__(256) template_kernel(const PathsArgs A) {
     const GraphView &g = A.g;
@@ -234,29 +278,50 @@ __global__ void __launch_bounds__(256) template_kernel(const PathsArgs A) {
     const int64_t warp = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = (static_cast<int64_t>(gridDim.x) * blockDim.x) >> 5;
     const int64_t nu = static_cast<int64_t>(*A.n_unique);
-    for (int64_t ui = warp; ui < nu; ui += nwarps) {
-        const int32_t vs = __ldg(A.ulist + ui);
-        const int64_t row = FILL ? A.t_off[ui] : 0;
-        int64_t n = 0;
-        if (__ldg(g.ntype + vs) == ET_SERVER) {
-            n += server_chunk<FILL>(A, row, lane == 0 ? vs : -1, -2, vs, 0, 0, lane);
-        } else {
-            const uint32_t s2 = __ldg(g.roff + vs), e2 = __ldg(g.roff + vs + 1);
-            for (uint32_t p2 = s2; p2 < e2; p2 += 32) {
-                const uint32_t k2 = p2 + lane;
-                int32_t srv = -1; int rsv = -1;
-                if (k2 < e2) {
-                    const uint32_t m2 = __ldg(g.rmeta + k2);
-                    if (!(m2 & ABB_META_REVERSED_COPY) && (m2 & ABB_META_REL_MASK) == REL_DEPENDS_ON) {
-                        const int32_t v2 = __ldg(g.rnbr + k2);
-                        if (__ldg(g.ntype + v2) == ET_SERVER) { srv = v2; rsv = (m2 & ABB_META_FIRST_PAIR) ? REL_DEPENDS_ON : -3; }
+    for (int64_t base = warp * 32; base < nu; base += nwarps * 32) {
+        const int64_t ui = base + lane;
+        int32_t vs = -1; uint32_t s2 = 0, e2 = 0; bool is_long = false;
+        int64_t row = 0, n = 0;
+        if (ui < nu) {
+            vs = __ldg(A.ulist + ui);
+            if (FILL) row = A.t_off[ui];
+            if (__ldg(g.ntype + vs) == ET_SERVER) {
+                n = server_rows(A, vs);
+                if (FILL) copy_server_rows(A, row, vs, vs, -2);
+            } else {
+                s2 = __ldg(g.roff + vs); e2 = __ldg(g.roff + vs + 1);
+                is_long = e2 - s2 > LONG_ROW;
+                if (!is_long) {
+                    for (uint32_t p = s2; p < e2; p++) {
+                        int rsv;
+                        const int32_t s = dependent_server(g, p, rsv);
+                        if (s < 0) continue;
+                        if (FILL) copy_server_rows(A, row + n, s, vs, rsv);
+                        n += server_rows(A, s);
                     }
                 }
-                if (FILL && rsv == -3) rsv = first_rel_rev(g, srv, vs);
-                if (__any_sync(FULL, srv >= 0)) n += server_chunk<FILL>(A, row + n, srv, rsv, vs, 0, 0, lane);
             }
         }
-        if (lane == 0) {
+        for (unsigned rem = __ballot_sync(FULL, is_long); rem; rem &= rem - 1) {
+            const int src = __ffs(rem) - 1;
+            const int32_t lvs = __shfl_sync(FULL, vs, src);
+            const uint32_t ls2 = __shfl_sync(FULL, s2, src), le2 = __shfl_sync(FULL, e2, src);
+            const int64_t lrow = __shfl_sync(FULL, row, src);
+            int64_t ln = 0;
+            for (uint32_t p = ls2; p < le2; p += 32) {
+                const uint32_t k = p + lane;
+                int rsv = -1;
+                const int32_t s = k < le2 ? dependent_server(g, k, rsv) : -1;
+                const int64_t c = s >= 0 ? server_rows(A, s) : 0;
+                int64_t inc = c;
+#pragma unroll
+                for (int o = 1; o < 32; o <<= 1) { const int64_t v = __shfl_up_sync(FULL, inc, o); if (lane >= o) inc += v; }
+                if (FILL && s >= 0) copy_server_rows(A, lrow + ln + inc - c, s, lvs, rsv);
+                ln += __shfl_sync(FULL, inc, 31);
+            }
+            if (lane == src) n = ln;
+        }
+        if (ui < nu) {
             if (!FILL) { A.t_cnt[ui] = n; A.t_cnt_node[vs] = static_cast<int32_t>(n); }
             else A.t_off_node[vs] = row;
         }
@@ -273,51 +338,104 @@ __global__ void finding_offsets_kernel(const PathsArgs A) {
     if (fi <= A.io.n_findings) A.io.f_off[fi] = A.link_roff[A.link_off[fi]];
 }
 
-// ---- pass C: every link copies its vulnerable source's template, substituting the finding
-__device__ __forceinline__ void emit_row(const PathsArgs &A, int64_t out, int64_t t, int32_t vs, int32_t f, int rel_vf) {
-    const int4 tr = A.t_row[t];
-    const int32_t srv = tr.y;
-    const int ras = A.t_rel[t * 2], rsv = A.t_rel[t * 2 + 1];
-    reinterpret_cast<int4 *>(A.io.hops)[out] = make_int4(tr.x, srv, (vs != srv) ? vs : -1, f);
-    // rels are stored 4 bytes per row (the 4th is padding) so a row's relationships are one aligned word
-    const uint32_t packed = (vs != srv) ? ((ras & 0xFF) | ((rsv & 0xFF) << 8) | ((rel_vf & 0xFF) << 16) | (0xFEu << 24))
-                                        : ((ras & 0xFF) | ((rel_vf & 0xFF) << 8) | (0xFEu << 16) | (0xFEu << 24));
-    reinterpret_cast<uint32_t *>(A.io.rels)[out] = packed;
-    A.io.ncred[out] = tr.z;
-    A.io.ntool[out] = tr.w;
+// ---- pass C: every link copies its vulnerable source's template, substituting the finding.
+// Row-parallel: the flat rows [0, R) are cut into tiles of ROW_TILE, and a block takes a contiguous run of tiles.  Warp w of the
+// block takes ROW_ITEMS * 32 consecutive rows of a tile, 32 at a time, so each output stream is written in whole coalesced lines.
+// The links of a tile are found in the block's shared copy of the link_roff window that starts at the tile's first link (ROW_WIN
+// links, stored relative to the tile's first row).  A warp carries its current link from step to step: a lane searches only when
+// its row lies past that link's end, which in long links (almost every row) is one shared-memory compare.  A tile that spans
+// more links than the window holds (a run of zero-row links) searches the rest in global memory.
+// The tile size and 6 resident blocks per SM for replicate_kernel are what measured fastest at L on the H100: a block's two
+// barriers and window load per tile are exposed latency, which larger tiles and more resident warps hide (unrolling steps to
+// keep more loads in flight per warp cost registers, hence occupancy, and did not help).
+constexpr int ROW_THREADS = 256, ROW_ITEMS = 32, ROW_TILE = ROW_THREADS * ROW_ITEMS, ROW_WIN = 1024;
+
+// last l in [lo, hi) with roff[l] <= r, given roff[lo] <= r
+template <class T, class I>
+__device__ __forceinline__ I last_le(const T *roff, I lo, I hi, T r) {
+    while (hi - lo > 1) { const I mid = (lo + hi) >> 1; if (roff[mid] <= r) lo = mid; else hi = mid; }
+    return lo;
 }
 
-__global__ void __launch_bounds__(256) replicate_kernel(const PathsArgs A) {
-    const int lane = threadIdx.x & 31;
-    const int64_t warp = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
-    const int64_t nwarps = (static_cast<int64_t>(gridDim.x) * blockDim.x) >> 5;
-    const int64_t nf = A.io.n_findings;
-    // a warp takes 32 findings; short links are copied lane-serially, long ones by the whole warp
-    for (int64_t fb = warp * 32; fb < nf; fb += nwarps * 32) {
-        const int64_t fi = fb + lane;
-        int64_t l0 = 0, l1 = 0; int32_t f = 0;
-        if (fi < nf) { l0 = A.link_off[fi]; l1 = A.link_off[fi + 1]; f = __ldg(A.io.findings + fi); }
-        for (int64_t l = l0; l < l1; l++) {
-            const int64_t rows = A.link_roff[l + 1] - A.link_roff[l];
-            if (rows > 8) continue;                 // long links below
-            const int32_t vs = A.link_vs[l]; const int rel = A.link_rel[l];
-            const int64_t t0 = A.t_off_node[vs], o0 = A.link_roff[l];
-            for (int64_t k = 0; k < rows; k++) emit_row(A, o0 + k, t0 + k, vs, f, rel);
+// Visits every flat row once as fn.store(row, fn.load(row, link)).  Every thread of the block must call it (ROW_THREADS per block).
+template <class Fn>
+__device__ __forceinline__ void for_each_row(const PathsArgs &A, const Fn &fn) {
+    __shared__ int32_t s_roff[ROW_WIN + 1];   // link_roff[l0 + i] - r0, clamped to [-1, ROW_TILE + 1]: exact for every comparison with a row of the tile
+    __shared__ int64_t s_l0;
+    const int lane = threadIdx.x & 31, w0 = (threadIdx.x >> 5) * ROW_ITEMS * 32;
+    const int64_t NL = static_cast<int64_t>(*A.n_links), R = A.link_roff[NL];
+    const int64_t ntiles = (R + ROW_TILE - 1) / ROW_TILE, per = (ntiles + gridDim.x - 1) / gridDim.x;
+    const int64_t tb = blockIdx.x * per, te = min(ntiles, tb + per);
+    if (tb >= te) return;
+    if (threadIdx.x == 0) s_l0 = last_le(A.link_roff, int64_t{0}, NL, tb * ROW_TILE);
+    for (int64_t tile = tb; tile < te; tile++) {
+        __syncthreads();
+        const int64_t l0 = s_l0, r0 = tile * ROW_TILE;
+        const int n = static_cast<int>(min(static_cast<int64_t>(ROW_TILE), R - r0));   // rows of this tile
+        const int nw = static_cast<int>(min(static_cast<int64_t>(ROW_WIN), NL - l0));  // window: links l0 .. l0+nw-1, bounds s_roff[0..nw]
+        for (int i = threadIdx.x; i <= nw; i += ROW_THREADS) {
+            const int64_t d = A.link_roff[l0 + i] - r0;
+            s_roff[i] = d < 0 ? -1 : static_cast<int32_t>(min(d, static_cast<int64_t>(ROW_TILE + 1)));
         }
-        // long links: lane j announces them one at a time, the warp streams the template 32 rows per step
-        for (int j = 0; j < 32; j++) {
-            const int64_t jl0 = __shfl_sync(FULL, l0, j), jl1 = __shfl_sync(FULL, l1, j);
-            const int32_t jf = __shfl_sync(FULL, f, j);
-            for (int64_t l = jl0; l < jl1; l++) {
-                const int64_t o0 = A.link_roff[l], rows = A.link_roff[l + 1] - o0;
-                if (rows <= 8) continue;
-                const int32_t vs = A.link_vs[l]; const int rel = A.link_rel[l];
-                const int64_t t0 = A.t_off_node[vs];
-                for (int64_t k = lane; k < rows; k += 32) emit_row(A, o0 + k, t0 + k, vs, jf, rel);
+        __syncthreads();
+        const int wend = s_roff[nw];   // tile rows below this lie in the window's links
+        int j = 0;                     // warp-uniform: window link of the warp's last row so far
+        for (int it = 0; it < ROW_ITEMS && w0 + it * 32 < n; it++) {
+            const int k = w0 + it * 32 + lane;
+            int jl = j;
+            if (k < n) {
+                int64_t l;
+                if (k < wend) {
+                    if (s_roff[jl + 1] <= k) jl = last_le(s_roff, jl + 1, nw, static_cast<int32_t>(k));
+                    l = l0 + jl;
+                } else {
+                    l = last_le(A.link_roff, l0 + nw, NL, r0 + k);
+                }
+                fn.store(r0 + k, fn.load(r0 + k, l));
             }
+            j = __shfl_sync(FULL, jl, 31);   // rows ascend with the lane; a partial step is the tile's last
         }
+        if (threadIdx.x == 0 && r0 + ROW_TILE < R)
+            s_l0 = ROW_TILE < wend ? l0 + last_le(s_roff, 0, nw, static_cast<int32_t>(ROW_TILE)) : last_le(A.link_roff, l0 + nw, NL, r0 + ROW_TILE);
     }
 }
+
+// what one flat row needs: its template row and relationships, and its link's vulnerable source, finding and (vs, finding) relationship
+struct RowValue {
+    int4 tr;
+    uint32_t rp;   // (agent,server) and (server,vs) relationships
+    int32_t vs, f, rel;
+};
+
+__device__ __forceinline__ RowValue row_value(const PathsArgs &A, int64_t t, int32_t vs, int32_t f, int rel) {
+    return RowValue{__ldg(A.t_row + t), __ldg(reinterpret_cast<const uint16_t *>(A.t_rel) + t), vs, f, rel};
+}
+
+// template row of flat row r of link l
+__device__ __forceinline__ int64_t template_row(const PathsArgs &A, int64_t r, int64_t l) { return __ldg(A.link_toff + l) + (r - __ldg(A.link_roff + l)); }
+
+__device__ __forceinline__ void emit_row(const PathsArgs &A, int64_t out, const RowValue &v) {
+    const int32_t srv = v.tr.y;
+    const uint32_t ras = v.rp & 0xFF, rsv = v.rp >> 8;
+    reinterpret_cast<int4 *>(A.io.hops)[out] = make_int4(v.tr.x, srv, (v.vs != srv) ? v.vs : -1, v.f);
+    // rels are stored 4 bytes per row (the 4th is padding) so a row's relationships are one aligned word
+    const uint32_t packed = (v.vs != srv) ? (ras | (rsv << 8) | ((v.rel & 0xFF) << 16) | (0xFEu << 24))
+                                          : (ras | ((v.rel & 0xFF) << 8) | (0xFEu << 16) | (0xFEu << 24));
+    reinterpret_cast<uint32_t *>(A.io.rels)[out] = packed;
+    A.io.ncred[out] = v.tr.z;
+    A.io.ntool[out] = v.tr.w;
+}
+
+struct ReplicateRows {
+    const PathsArgs &A;
+    using Value = RowValue;
+    __device__ __forceinline__ Value load(int64_t r, int64_t l) const {
+        return row_value(A, template_row(A, r, l), __ldg(A.link_vs + l), __ldg(A.io.findings + __ldg(A.link_f + l)), __ldg(A.link_rel + l));
+    }
+    __device__ __forceinline__ void store(int64_t r, const Value &v) const { emit_row(A, r, v); }
+};
+
+__global__ void __launch_bounds__(ROW_THREADS, 6) replicate_kernel(const PathsArgs A) { for_each_row(A, ReplicateRows{A}); }
 
 
 // ---- ranking (reference api/routes/graph.py:762-786): sort key of every row, then the requested page is gathered.
@@ -332,42 +450,24 @@ struct RankArgs {
     uint32_t *rows;               // [n_rows] row index
 };
 
-__device__ __forceinline__ unsigned long long rank_key(const PathsArgs &A, const RankArgs &R, int64_t fi, int64_t t, int32_t vs) {
-    const int4 tr = A.t_row[t];
-    const int nc = tr.z < 4 ? tr.z : 4, nt = tr.w < 14 ? tr.w : 14;
-    const unsigned long long rr = R.risk_rank[(static_cast<int64_t>(R.base_id[fi]) * 5 + nc) * 15 + nt];
-    const unsigned long long nh = (vs != tr.y) ? 4ull : 3ull;
-    const unsigned long long cu = static_cast<unsigned long long>(min(R.ncu[tr.y], 0x3FFFF)), tu = static_cast<unsigned long long>(min(R.ntu[tr.y], 0x3FFFF));
-    return ~((rr << 40) | (nh << 36) | (cu << 18) | tu);
-}
-
-__global__ void __launch_bounds__(256) rank_keys_kernel(const PathsArgs A, const RankArgs R) {
-    const int lane = threadIdx.x & 31;
-    const int64_t warp = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
-    const int64_t nwarps = (static_cast<int64_t>(gridDim.x) * blockDim.x) >> 5;
-    const int64_t nf = A.io.n_findings;
-    for (int64_t fb = warp * 32; fb < nf; fb += nwarps * 32) {
-        const int64_t fi = fb + lane;
-        int64_t l0 = 0, l1 = 0;
-        if (fi < nf) { l0 = A.link_off[fi]; l1 = A.link_off[fi + 1]; }
-        for (int64_t l = l0; l < l1; l++) {
-            const int64_t o0 = A.link_roff[l], rows = A.link_roff[l + 1] - o0;
-            if (rows > 8) continue;
-            const int32_t vs = A.link_vs[l]; const int64_t t0 = A.t_off_node[vs];
-            for (int64_t k = 0; k < rows; k++) { R.keys[o0 + k] = rank_key(A, R, fi, t0 + k, vs); R.rows[o0 + k] = static_cast<uint32_t>(o0 + k); }
-        }
-        for (int j = 0; j < 32; j++) {
-            const int64_t jl0 = __shfl_sync(FULL, l0, j), jl1 = __shfl_sync(FULL, l1, j);
-            const int64_t jfi = fb + j;
-            for (int64_t l = jl0; l < jl1; l++) {
-                const int64_t o0 = A.link_roff[l], rows = A.link_roff[l + 1] - o0;
-                if (rows <= 8) continue;
-                const int32_t vs = A.link_vs[l]; const int64_t t0 = A.t_off_node[vs];
-                for (int64_t k = lane; k < rows; k += 32) { R.keys[o0 + k] = rank_key(A, R, jfi, t0 + k, vs); R.rows[o0 + k] = static_cast<uint32_t>(o0 + k); }
-            }
-        }
+struct RankRows {
+    const PathsArgs &A;
+    const RankArgs &R;
+    struct Value { int4 tr; int32_t fi, vs; };
+    __device__ __forceinline__ Value load(int64_t r, int64_t l) const {
+        return Value{__ldg(A.t_row + template_row(A, r, l)), __ldg(A.link_f + l), __ldg(A.link_vs + l)};
     }
-}
+    __device__ __forceinline__ void store(int64_t r, const Value &v) const {
+        const int nc = v.tr.z < 4 ? v.tr.z : 4, nt = v.tr.w < 14 ? v.tr.w : 14;
+        const unsigned long long rr = R.risk_rank[(static_cast<int64_t>(R.base_id[v.fi]) * 5 + nc) * 15 + nt];
+        const unsigned long long nh = (v.vs != v.tr.y) ? 4ull : 3ull;
+        const unsigned long long cu = static_cast<unsigned long long>(min(R.ncu[v.tr.y], 0x3FFFF)), tu = static_cast<unsigned long long>(min(R.ntu[v.tr.y], 0x3FFFF));
+        R.keys[r] = ~((rr << 40) | (nh << 36) | (cu << 18) | tu);
+        R.rows[r] = static_cast<uint32_t>(r);
+    }
+};
+
+__global__ void __launch_bounds__(ROW_THREADS) rank_keys_kernel(const PathsArgs A, const RankArgs R) { for_each_row(A, RankRows{A, R}); }
 
 // the page [first, first+count) of the sorted order -> flat rows (+ the risk rank so the host can print the float)
 __global__ void rank_gather_kernel(const PathsArgs A, const RankArgs R, const uint32_t *sorted_rows, int64_t first, int64_t count, uint32_t *out_rank,
@@ -384,8 +484,9 @@ __global__ void rank_gather_kernel(const PathsArgs A, const RankArgs R, const ui
     const int64_t l = a;
     const int32_t vs = A.link_vs[l];
     const int64_t t = A.t_off_node[vs] + (row - A.link_roff[l]);
-    emit_row(A, i, t, vs, A.io.findings[fi], A.link_rel[l]);
-    const int4 tr = A.t_row[t];
+    const RowValue v = row_value(A, t, vs, A.io.findings[fi], A.link_rel[l]);
+    emit_row(A, i, v);
+    const int4 tr = v.tr;
     const int nc = tr.z < 4 ? tr.z : 4, nt = tr.w < 14 ? tr.w : 14;
     out_rank[i] = R.risk_rank[(static_cast<int64_t>(R.base_id[fi]) * 5 + nc) * 15 + nt];
     out_row[i] = row;
