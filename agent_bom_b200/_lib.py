@@ -62,6 +62,8 @@ class PathsIO(C.Structure):
 WALK_TRAVERSABLE_ONLY, WALK_MARK_ROOTS, WALK_OMIT_ROOTS, WALK_PARENTS, WALK_DEPTHS = 0x1, 0x2, 0x4, 0x8, 0x10
 WALK_EDGES, WALK_HIST, WALK_REAL_ROOTS, WALK_TARGET = 0x20, 0x40, 0x80, 0x100
 QFLAG_TRUNCATED, QFLAG_NO_ROOT, QFLAG_TARGET_FOUND = 1, 2, 4
+# focus bits of the fix-first ranking (include/abb200.h, table in csrc/paths.cuh)
+FOCUS_CVE, FOCUS_CVE_FINDING, FOCUS_PACKAGE, FOCUS_AGENT = 0x1, 0x2, 0x4, 0x8
 DIR_FORWARD, DIR_REVERSE, DIR_BOTH = 1, 2, 3
 
 #: every symbol include/abb200.h declares (tests assert the .so exports all of them)
@@ -134,6 +136,8 @@ EXPORTS = {
     "abb_paths_result_d2h_bytes": (i64, [vp]),
     "abb_paths_result_free": (None, [vp]),
     "abb_paths_rank_host": (C.c_int, [vp, vp, i64, vp, vp, i64, vp, vp, i64, i64, C.POINTER(vp)]),
+    "abb_paths_rank_focus_host": (C.c_int, [vp, vp, i64, vp, vp, i64, vp, vp, vp, u32, i64, i64, C.POINTER(vp)]),
+    "abb_rank_result_matched": (i64, [vp]),
     "abb_rank_result_total": (i64, [vp]),
     "abb_rank_result_count": (i64, [vp]),
     "abb_rank_result_hops": (vp, [vp]),

@@ -1589,7 +1589,7 @@ extern "C" int abb_paths_host(abb_graph *g, const int32_t *findings, int64_t n_f
 
 // ------------------------------------------------------------------ ranked page of exposure-path rows
 struct abb_rank_result {
-    int64_t total = 0, count = 0;
+    int64_t total = 0, matched = 0, count = 0;
     std::vector<int32_t> hops, ncred, ntool;
     std::vector<int8_t> rels;
     std::vector<uint32_t> risk_rank;
@@ -1598,6 +1598,7 @@ struct abb_rank_result {
 extern "C" void abb_rank_result_free(abb_rank_result *r) { delete r; }
 extern "C" int64_t abb_rank_result_total(const abb_rank_result *r) { return r->total; }
 extern "C" int64_t abb_rank_result_count(const abb_rank_result *r) { return r->count; }
+extern "C" int64_t abb_rank_result_matched(const abb_rank_result *r) { return r->matched; }
 extern "C" const int32_t *abb_rank_result_hops(const abb_rank_result *r) { return r->hops.data(); }
 extern "C" const int8_t *abb_rank_result_rels(const abb_rank_result *r) { return r->rels.data(); }
 extern "C" const int32_t *abb_rank_result_ncred(const abb_rank_result *r) { return r->ncred.data(); }
@@ -1615,22 +1616,27 @@ struct ScopedDev {   // scoped device allocation for the ranking pass (sizes fol
     template <class T> T *as() const { return static_cast<T *>(p); }
 };
 
-extern "C" int abb_paths_rank_host(abb_graph *g, const int32_t *findings, int64_t n_findings, const int32_t *base_id, const uint32_t *risk_rank, int64_t n_base,
-                                   const int32_t *ncu, const int32_t *ntu, int64_t offset, int64_t limit, abb_rank_result **out) {
-    NvtxRange nvtx_("abb_paths_rank_host");
+// One ranking path: node_focus == nullptr ranks every row (abb_paths_rank_host); otherwise the rows that miss the focus are
+// compacted away (cub::DeviceSelect keeps their order) and only the matched rows are sorted.
+static int paths_rank(abb_graph *g, const int32_t *findings, int64_t n_findings, const int32_t *base_id, const uint32_t *risk_rank, int64_t n_base,
+                      const int32_t *ncu, const int32_t *ntu, const uint8_t *node_focus, uint32_t need, int64_t offset, int64_t limit,
+                      abb_rank_result **out) {
     if (!g || !out || n_findings < 0 || offset < 0 || limit < 0 || n_base <= 0 || !risk_rank || !ncu || !ntu || (n_findings && (!findings || !base_id)))
         return fail(ABB_ERR_ARG, "bad arguments");
+    if (node_focus && (need & ~(ABB_FOCUS_CVE | ABB_FOCUS_PACKAGE | ABB_FOCUS_AGENT))) return fail(ABB_ERR_ARG, "need: unknown focus category 0x%x", need);
     DeviceGuard dg(g->device);
     std::lock_guard<std::mutex> lk(g->mu);
     cudaStream_t st = g->stream;
     const int64_t nf = n_findings, n = g->v.n;
+    const bool focused = node_focus != nullptr;
     if (int rc = g->p_findings.ensure(static_cast<size_t>(nf + 1) * 4)) return rc;
     if (int rc = g->p_off.ensure(static_cast<size_t>(nf + 1) * 8)) return rc;
-    ScopedDev d_base, d_tab, d_ncu, d_ntu;
+    ScopedDev d_base, d_tab, d_ncu, d_ntu, d_focus;
     if (int rc = d_base.alloc(static_cast<size_t>(nf + 1) * 4)) return rc;
     if (int rc = d_tab.alloc(static_cast<size_t>(n_base) * 75 * 4)) return rc;
     if (int rc = d_ncu.alloc(static_cast<size_t>(n + 1) * 4)) return rc;
     if (int rc = d_ntu.alloc(static_cast<size_t>(n + 1) * 4)) return rc;
+    if (focused) { if (int rc = d_focus.alloc(static_cast<size_t>(n + 1))) return rc; }
     if (nf) {
         CUDA_TRY(cudaMemcpyAsync(g->p_findings.p, findings, static_cast<size_t>(nf) * 4, cudaMemcpyHostToDevice, st));
         CUDA_TRY(cudaMemcpyAsync(d_base.p, base_id, static_cast<size_t>(nf) * 4, cudaMemcpyHostToDevice, st));
@@ -1638,6 +1644,7 @@ extern "C" int abb_paths_rank_host(abb_graph *g, const int32_t *findings, int64_
     CUDA_TRY(cudaMemcpyAsync(d_tab.p, risk_rank, static_cast<size_t>(n_base) * 75 * 4, cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(d_ncu.p, ncu, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(d_ntu.p, ntu, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, st));
+    if (focused) CUDA_TRY(cudaMemcpyAsync(d_focus.p, node_focus, static_cast<size_t>(n), cudaMemcpyHostToDevice, st));
     abb_paths_io io{};
     io.n_findings = nf; io.findings = g->p_findings.as<int32_t>(); io.f_off = g->p_off.as<int64_t>();
     if (int rc = enqueue_paths_count(g, &io, st)) return rc;
@@ -1647,34 +1654,60 @@ extern "C" int abb_paths_rank_host(abb_graph *g, const int32_t *findings, int64_
     if (R >= (1ll << 32) - 1) return fail(ABB_ERR_CAPACITY, "more than 2^32 exposure-path rows in one ranking batch");
     abb_rank_result *r = new abb_rank_result();
     r->total = R;
-    const int64_t first = std::min(offset, R), count = std::min(limit, R - first);
-    r->count = count;
-    if (R == 0 || count == 0) { *out = r; return ABB_OK; }
-    ScopedDev k1, k2, v1, v2, tmp, o_hops, o_rels, o_nc, o_nt, o_rank, o_row;
+    r->matched = R;
+    // unfocused, the page is known before any kernel runs; focused, the matched count is needed first
+    if (R == 0 || (!focused && std::min(limit, R - std::min(offset, R)) == 0)) { r->matched = focused ? 0 : R; *out = r; return ABB_OK; }
+    ScopedDev k1, k2, v1, v2, tmp, d_sel, sel_tmp;
     int rc = k1.alloc(static_cast<size_t>(R) * 8);
     if (!rc) rc = k2.alloc(static_cast<size_t>(R) * 8);
     if (!rc) rc = v1.alloc(static_cast<size_t>(R) * 4);
     if (!rc) rc = v2.alloc(static_cast<size_t>(R) * 4);
-    if (!rc) rc = o_hops.alloc(static_cast<size_t>(count) * 16);
+    if (rc) { delete r; return rc; }
+    PathsArgs A = g->paths_args;
+    RankArgs RA{d_base.as<int32_t>(), d_tab.as<uint32_t>(), d_ncu.as<int32_t>(), d_ntu.as<int32_t>(), k1.as<unsigned long long>(), v1.as<uint32_t>(),
+                d_focus.as<uint8_t>(), io.findings, need};
+    rank_keys_kernel<<<row_grid(g, rank_keys_kernel, g->rank_keys_grid), ROW_THREADS, 0, st>>>(A, RA); g_launches++;
+    // sort input: every row (k1, v1), or the matched rows compacted into (k2, v2); the sorted pairs land in the other pair
+    unsigned long long *key_in = k1.as<unsigned long long>(), *key_out = k2.as<unsigned long long>();
+    uint32_t *row_in = v1.as<uint32_t>(), *row_out = v2.as<uint32_t>();
+    cudaError_t ce = cudaSuccess;
+    size_t tb = 0;
+    if (focused) {
+        if (!(rc = d_sel.alloc(8))) {
+            ce = cub::DeviceSelect::If(nullptr, tb, v1.as<uint32_t>(), v2.as<uint32_t>(), d_sel.as<int64_t>(), static_cast<int>(R), RowMatched{}, st);
+            if (ce == cudaSuccess && !(rc = sel_tmp.alloc(tb)))
+                ce = cub::DeviceSelect::If(sel_tmp.p, tb, v1.as<uint32_t>(), v2.as<uint32_t>(), d_sel.as<int64_t>(), static_cast<int>(R), RowMatched{}, st);
+            g_launches++;
+        }
+        int64_t M = 0;
+        if (!rc && ce == cudaSuccess) ce = cudaMemcpyAsync(&M, d_sel.p, 8, cudaMemcpyDeviceToHost, st);
+        if (!rc && ce == cudaSuccess) ce = cudaStreamSynchronize(st);
+        if (rc || ce != cudaSuccess) { delete r; return rc ? rc : fail(ABB_ERR_CUDA, "focus compaction failed: %s", cudaGetErrorString(ce)); }
+        r->matched = M;
+        if (M == 0 || std::min(limit, M - std::min(offset, M)) == 0) { *out = r; return ABB_OK; }
+        gather_keys_kernel<<<static_cast<unsigned>((M + 255) / 256), 256, 0, st>>>(k1.as<unsigned long long>(), v2.as<uint32_t>(), M, k2.as<unsigned long long>());
+        g_launches++;
+        std::swap(key_in, key_out); std::swap(row_in, row_out);
+    }
+    const int64_t M = r->matched;
+    const int64_t first = std::min(offset, M), count = std::min(limit, M - first);
+    r->count = count;
+    tb = 0;
+    ce = cub::DeviceRadixSort::SortPairs(nullptr, tb, key_in, key_out, row_in, row_out, static_cast<int>(M), 0, 64, st);
+    if (ce == cudaSuccess && !(rc = tmp.alloc(tb)))
+        ce = cub::DeviceRadixSort::SortPairs(tmp.p, tb, key_in, key_out, row_in, row_out, static_cast<int>(M), 0, 64, st);
+    g_launches++;
+    if (rc || ce != cudaSuccess) { delete r; return rc ? rc : fail(ABB_ERR_CUDA, "radix sort failed: %s", cudaGetErrorString(ce)); }
+    ScopedDev o_hops, o_rels, o_nc, o_nt, o_rank, o_row;
+    rc = o_hops.alloc(static_cast<size_t>(count) * 16);
     if (!rc) rc = o_rels.alloc(static_cast<size_t>(count) * 4);
     if (!rc) rc = o_nc.alloc(static_cast<size_t>(count) * 4);
     if (!rc) rc = o_nt.alloc(static_cast<size_t>(count) * 4);
     if (!rc) rc = o_rank.alloc(static_cast<size_t>(count) * 4);
     if (!rc) rc = o_row.alloc(static_cast<size_t>(count) * 8);
     if (rc) { delete r; return rc; }
-    PathsArgs A = g->paths_args;
-    RankArgs RA{d_base.as<int32_t>(), d_tab.as<uint32_t>(), d_ncu.as<int32_t>(), d_ntu.as<int32_t>(), k1.as<unsigned long long>(), v1.as<uint32_t>()};
-    rank_keys_kernel<<<row_grid(g, rank_keys_kernel, g->rank_keys_grid), ROW_THREADS, 0, st>>>(A, RA); g_launches++;
-    size_t tb = 0;
-    cudaError_t ce = cub::DeviceRadixSort::SortPairs(nullptr, tb, k1.as<unsigned long long>(), k2.as<unsigned long long>(), v1.as<uint32_t>(), v2.as<uint32_t>(),
-                                                     static_cast<int>(R), 0, 64, st);
-    if (ce == cudaSuccess && !(rc = tmp.alloc(tb)))
-        ce = cub::DeviceRadixSort::SortPairs(tmp.p, tb, k1.as<unsigned long long>(), k2.as<unsigned long long>(), v1.as<uint32_t>(), v2.as<uint32_t>(),
-                                             static_cast<int>(R), 0, 64, st);
-    g_launches++;
-    if (rc || ce != cudaSuccess) { delete r; return rc ? rc : fail(ABB_ERR_CUDA, "radix sort failed: %s", cudaGetErrorString(ce)); }
     A.io.hops = o_hops.as<int32_t>(); A.io.rels = o_rels.as<int8_t>(); A.io.ncred = o_nc.as<int32_t>(); A.io.ntool = o_nt.as<int32_t>(); A.io.row_cap = count;
-    rank_gather_kernel<<<static_cast<unsigned>((count + 255) / 256), 256, 0, st>>>(A, RA, v2.as<uint32_t>(), first, count, o_rank.as<uint32_t>(), o_row.as<int64_t>());
+    rank_gather_kernel<<<static_cast<unsigned>((count + 255) / 256), 256, 0, st>>>(A, RA, row_out, first, count, o_rank.as<uint32_t>(), o_row.as<int64_t>());
     g_launches++;
     r->hops.resize(static_cast<size_t>(count) * 4); r->rels.resize(static_cast<size_t>(count) * 4); r->ncred.resize(count); r->ntool.resize(count);
     r->risk_rank.resize(count); r->row.resize(count);
@@ -1689,6 +1722,19 @@ extern "C" int abb_paths_rank_host(abb_graph *g, const int32_t *findings, int64_
     if (ce != cudaSuccess) { delete r; return fail(ABB_ERR_CUDA, "ranking failed: %s", cudaGetErrorString(ce)); }
     *out = r;
     return ABB_OK;
+}
+
+extern "C" int abb_paths_rank_host(abb_graph *g, const int32_t *findings, int64_t n_findings, const int32_t *base_id, const uint32_t *risk_rank, int64_t n_base,
+                                   const int32_t *ncu, const int32_t *ntu, int64_t offset, int64_t limit, abb_rank_result **out) {
+    NvtxRange nvtx_("abb_paths_rank_host");
+    return paths_rank(g, findings, n_findings, base_id, risk_rank, n_base, ncu, ntu, nullptr, 0, offset, limit, out);
+}
+
+extern "C" int abb_paths_rank_focus_host(abb_graph *g, const int32_t *findings, int64_t n_findings, const int32_t *base_id, const uint32_t *risk_rank,
+                                         int64_t n_base, const int32_t *ncu, const int32_t *ntu, const uint8_t *node_focus, uint32_t need, int64_t offset,
+                                         int64_t limit, abb_rank_result **out) {
+    NvtxRange nvtx_("abb_paths_rank_focus_host");
+    return paths_rank(g, findings, n_findings, base_id, risk_rank, n_base, ncu, ntu, node_focus, need, offset, limit, out);
 }
 
 extern "C" int abb_exposure_host(abb_graph *g, const int32_t *findings, int64_t n_findings, int32_t max_depth, abb_walk_result **impact_out,

@@ -441,14 +441,42 @@ __global__ void __launch_bounds__(ROW_THREADS, 6) replicate_kernel(const PathsAr
 // ---- ranking (reference api/routes/graph.py:762-786): sort key of every row, then the requested page is gathered.
 // key (descending) = (risk rank, #hops, #distinct credential labels, #distinct tool labels); ties keep emission order
 // (Python's stable sort with reverse=True) — the radix sort below is stable on the complemented key.
+//
+// Focus (the fix-first view's cve / package / agent filter, reference _path_matches_focus, api/routes/graph.py:448-476).  The
+// host passes one byte per node; norm(s) = s.strip().lower(), computed on the host with Python string semantics, and nodes
+// without a record (ghosts) get 0:
+//
+//   bit                  set on node u when                                                          checked at hop
+//   ABB_FOCUS_CVE        norm(u.label) == cve_n, or u is VULNERABILITY / MISCONFIGURATION              any hop
+//                        and norm(u.label or u.id) == cve_n
+//   ABB_FOCUS_CVE_FINDING norm((u.label or u.id).strip()) == cve_n  (the path's vuln_ids entry)       the finding hop only
+//   ABB_FOCUS_PACKAGE    u is PACKAGE and norm(u.label or u.id) == package_n                          any hop
+//   ABB_FOCUS_AGENT      u is AGENT / USER / GROUP / SERVICE_ACCOUNT and norm(u.label or u.id) == agent_n  any hop
+//
+// The asymmetry is the reference's: the cve test looks at every hop's bare label, but at `label or id` only for finding-typed
+// hops and the path's own vuln_ids.  A row (agent, server, vulnerable source, finding) matches when every category named in
+// `need` (ABB_FOCUS_CVE / _PACKAGE / _AGENT; a CVE_FINDING bit on the finding counts as CVE) is set on at least one of its hops.
+// A focused pass writes row = ~0u for rows that do not match; they are compacted away (order preserved) before the sort.
 struct RankArgs {
     const int32_t *base_id;       // [n_findings] index of the finding's base risk value
     const uint32_t *risk_rank;    // [n_base * 5 * 15] dense rank of round(min(100, base + min(10, 3c) + min(10, .75t)), 2), c<=4, t<=14
     const int32_t *ncu;           // [n_nodes] distinct credential labels of a server
     const int32_t *ntu;           // [n_nodes] distinct tool labels of a server
     unsigned long long *keys;     // [n_rows] complemented sort key
-    uint32_t *rows;               // [n_rows] row index
+    uint32_t *rows;               // [n_rows] row index, ~0u when the row misses the focus
+    const uint8_t *focus;         // [n_nodes] focus bits of every node, or nullptr: every row matches
+    const int32_t *findings;      // [n_findings] finding node of each finding index (focused pass only)
+    uint32_t need;                // categories every matching row must satisfy
 };
+
+constexpr uint32_t ROW_UNMATCHED = 0xFFFFFFFFu;
+
+__device__ __forceinline__ bool row_matches(const RankArgs &R, int32_t agent, int32_t server, int32_t vs, int32_t f) {
+    const uint32_t on_hops = (__ldg(R.focus + agent) | __ldg(R.focus + server) | __ldg(R.focus + vs)) & ~ABB_FOCUS_CVE_FINDING;
+    const uint32_t on_f = __ldg(R.focus + f);
+    const uint32_t got = on_hops | on_f | ((on_f & ABB_FOCUS_CVE_FINDING) ? ABB_FOCUS_CVE : 0u);
+    return (got & R.need) == R.need;
+}
 
 struct RankRows {
     const PathsArgs &A;
@@ -463,11 +491,23 @@ struct RankRows {
         const unsigned long long nh = (v.vs != v.tr.y) ? 4ull : 3ull;
         const unsigned long long cu = static_cast<unsigned long long>(min(R.ncu[v.tr.y], 0x3FFFF)), tu = static_cast<unsigned long long>(min(R.ntu[v.tr.y], 0x3FFFF));
         R.keys[r] = ~((rr << 40) | (nh << 36) | (cu << 18) | tu);
-        R.rows[r] = static_cast<uint32_t>(r);
+        const bool hit = !R.focus || row_matches(R, v.tr.x, v.tr.y, v.vs, __ldg(R.findings + v.fi));
+        R.rows[r] = hit ? static_cast<uint32_t>(r) : ROW_UNMATCHED;
     }
 };
 
 __global__ void __launch_bounds__(ROW_THREADS) rank_keys_kernel(const PathsArgs A, const RankArgs R) { for_each_row(A, RankRows{A, R}); }
+
+// cub::DeviceSelect predicate of the focused pass
+struct RowMatched {
+    __host__ __device__ __forceinline__ bool operator()(uint32_t row) const { return row != ROW_UNMATCHED; }
+};
+
+// keys of the compacted rows (their rows ascend, so the stable sort still breaks ties in emission order)
+__global__ void gather_keys_kernel(const unsigned long long *keys, const uint32_t *rows, int64_t n, unsigned long long *out) {
+    const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = keys[rows[i]];
+}
 
 // the page [first, first+count) of the sorted order -> flat rows (+ the risk rank so the host can print the float)
 __global__ void rank_gather_kernel(const PathsArgs A, const RankArgs R, const uint32_t *sorted_rows, int64_t first, int64_t count, uint32_t *out_rank,

@@ -401,15 +401,28 @@ class DeviceGraph:
 
     def rank_exposure_paths(self, findings, base_id, risk_rank, ncu, ntu, offset: int = 0, limit: int = 100):
         """Page [offset, offset+limit) of the exposure-path rows in the reference's ranking order; returns (PathRows-like, risk_rank, total)."""
+        rows, rank, total, _matched = self.rank_exposure_paths_focused(findings, base_id, risk_rank, ncu, ntu, None, 0, offset, limit)
+        return rows, rank, total
+
+    def rank_exposure_paths_focused(self, findings, base_id, risk_rank, ncu, ntu, node_focus, need: int, offset: int = 0, limit: int = 100):
+        """Like ``rank_exposure_paths``, restricted to the rows whose hops carry every focus category in ``need``
+        (``node_focus``: uint8 ``_lib.FOCUS_*`` bits per node, ``None`` = every row).  The page is taken from the matched rows in
+        ranking order; returns (PathRows-like, risk_rank, total rows, matched rows)."""
         lib = _lib.load()
         f, b = _i32(findings), _i32(base_id)
         table = np.ascontiguousarray(risk_rank, dtype=np.uint32)
         cu, tu = _i32(ncu), _i32(ntu)
         assert table.size % 75 == 0 and cu.shape[0] == self.n_nodes and tu.shape[0] == self.n_nodes and b.shape[0] == f.shape[0]
+        focus = None if node_focus is None else np.ascontiguousarray(node_focus, dtype=np.uint8)
+        assert focus is None or focus.shape[0] == self.n_nodes
         res = _vp()
         with self._use() as h:
-            _lib.check(lib.abb_paths_rank_host(h, f.ctypes.data, int(f.shape[0]), b.ctypes.data, table.ctypes.data, table.size // 75, cu.ctypes.data,
-                                               tu.ctypes.data, int(offset), int(limit), C.byref(res)))
+            if focus is None:
+                _lib.check(lib.abb_paths_rank_host(h, f.ctypes.data, int(f.shape[0]), b.ctypes.data, table.ctypes.data, table.size // 75, cu.ctypes.data,
+                                                   tu.ctypes.data, int(offset), int(limit), C.byref(res)))
+            else:
+                _lib.check(lib.abb_paths_rank_focus_host(h, f.ctypes.data, int(f.shape[0]), b.ctypes.data, table.ctypes.data, table.size // 75,
+                                                         cu.ctypes.data, tu.ctypes.data, focus.ctypes.data, int(need), int(offset), int(limit), C.byref(res)))
         try:
             k = int(lib.abb_rank_result_count(res))
             rows = PathRows(
@@ -417,7 +430,7 @@ class DeviceGraph:
                 rels=np.ascontiguousarray(_view(lib.abb_rank_result_rels(res), k * 4, np.int8).reshape(k, 4)[:, :3]),
                 ncred=_view(lib.abb_rank_result_ncred(res), k, np.int32), ntool=_view(lib.abb_rank_result_ntool(res), k, np.int32),
             )
-            return rows, _view(lib.abb_rank_result_risk_rank(res), k, np.uint32), int(lib.abb_rank_result_total(res))
+            return rows, _view(lib.abb_rank_result_risk_rank(res), k, np.uint32), int(lib.abb_rank_result_total(res)), int(lib.abb_rank_result_matched(res))
         finally:
             lib.abb_rank_result_free(res)
 

@@ -66,6 +66,10 @@ class UnifiedGraph:
         self.device = device
         self._csr: csrmod.HostCSR | None = None
         self._dg = None
+        # per-graph caches of the ranked views (graph/exposure.py, graph/fix_first.py), dropped with the device graph
+        self._rank_inputs = None
+        self._focus_index = None
+        self._edge_lookup = None
 
     # ── construction from foreign graphs ────────────────────────────────
     @classmethod
@@ -85,6 +89,7 @@ class UnifiedGraph:
     # ── mutation (reference container.py:116-198) ───────────────────────
     def _invalidate(self) -> None:
         self._csr = None
+        self._rank_inputs = self._focus_index = self._edge_lookup = None
         if self._dg is not None:
             self._dg.close()
             self._dg = None
@@ -96,6 +101,7 @@ class UnifiedGraph:
             self.nodes[node.id] = node
             self._invalidate()
             return
+        self._rank_inputs = None          # a merge can raise severity / risk, which the ranking reads
         existing.last_seen = getattr(node, "last_seen", "") or _now_iso()
         existing.attributes.update(node.attributes)
         if SEVERITY_RANK.get(node.severity, 0) > SEVERITY_RANK.get(existing.severity, 0):

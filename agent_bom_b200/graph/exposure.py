@@ -101,6 +101,38 @@ def _server_label_counts(graph) -> tuple[np.ndarray, np.ndarray]:
     return counts[0::2][:n].astype(np.int32), counts[1::2][:n].astype(np.int32)
 
 
+class RankInputs:
+    """What the device ranking needs besides the topology, for one finding list: finding indices, per finding the index of its
+    base risk, the dense-rank table of every rounded score, and per server the distinct credential / tool label counts."""
+
+    __slots__ = ("idx", "base_id", "table", "ncu", "ntu")
+
+    def __init__(self, graph, finding_ids):
+        self.idx = np.asarray([graph.csr.idx(f) for f in finding_ids], dtype=np.int32)
+        base = np.asarray([node_risk_100(graph.nodes[f]) for f in finding_ids], dtype=np.float64)
+        base_vals, base_id = np.unique(base, return_inverse=True) if len(base) else (np.zeros(1), np.zeros(0, dtype=np.int64))
+        scores = np.empty((len(base_vals), 5, 15), dtype=np.float64)
+        for bi, b in enumerate(base_vals.tolist()):
+            for nc in range(5):
+                for nt in range(15):
+                    risk = b
+                    risk += min(10.0, nc * 3.0)
+                    risk += min(10.0, nt * 0.75)
+                    scores[bi, nc, nt] = round(min(100.0, risk), 2)
+        levels = np.unique(scores)
+        self.base_id = base_id.astype(np.int32)
+        self.table = np.searchsorted(levels, scores).astype(np.uint32)
+        self.ncu, self.ntu = _server_label_counts(graph)
+
+
+def rank_inputs(graph) -> RankInputs:
+    """The ranking inputs of every finding node, built once per graph (millions of ``node_risk_100`` calls and a label
+    de-duplication over every credential / tool edge at L) and dropped with the device graph."""
+    if getattr(graph, "_rank_inputs", None) is None:
+        graph._rank_inputs = RankInputs(graph, graph.finding_ids())
+    return graph._rank_inputs
+
+
 def ranked_attack_paths(graph, offset: int = 0, limit: int = 100, finding_ids=None) -> tuple[list[AttackPath], int]:
     """One page of the derived attack paths in the reference's order, ranked on the device (nothing but the page is materialised).
 
@@ -110,23 +142,8 @@ def ranked_attack_paths(graph, offset: int = 0, limit: int = 100, finding_ids=No
     if graph.attack_paths:
         paths = list(graph.attack_paths)
         return paths[offset: offset + limit], len(paths)
-    if finding_ids is None:
-        finding_ids = graph.finding_ids()
-    idx = np.asarray([graph.csr.idx(f) for f in finding_ids], dtype=np.int32)
-    base = np.asarray([node_risk_100(graph.nodes[f]) for f in finding_ids], dtype=np.float64)
-    base_vals, base_id = np.unique(base, return_inverse=True) if len(base) else (np.zeros(1), np.zeros(0, dtype=np.int64))
-    scores = np.empty((len(base_vals), 5, 15), dtype=np.float64)
-    for bi, b in enumerate(base_vals.tolist()):
-        for nc in range(5):
-            for nt in range(15):
-                risk = b
-                risk += min(10.0, nc * 3.0)
-                risk += min(10.0, nt * 0.75)
-                scores[bi, nc, nt] = round(min(100.0, risk), 2)
-    levels = np.unique(scores)
-    table = np.searchsorted(levels, scores).astype(np.uint32)
-    ncu, ntu = _server_label_counts(graph)
-    rows, _rank, total = graph.device_graph.rank_exposure_paths(idx, base_id.astype(np.int32), table, ncu, ntu, offset, limit)
+    ri = rank_inputs(graph) if finding_ids is None else RankInputs(graph, finding_ids)
+    rows, _rank, total = graph.device_graph.rank_exposure_paths(ri.idx, ri.base_id, ri.table, ri.ncu, ri.ntu, offset, limit)
     return materialize_attack_paths(graph, rows, sort=False), total
 
 

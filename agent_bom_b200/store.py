@@ -14,7 +14,7 @@ Conventions kept: keyword-only arguments; a missing snapshot / node yields
 ``None`` / ``([], set())`` / an empty graph, never an exception; methods are
 thread-safe (REST calls arrive on worker threads via ``asyncio.to_thread``).
 Batched extensions (``impact_of_many``, ``exposure_paths_many``,
-``dependency_reach``) expose what a GPU is actually good at.
+``fix_first_view``, ``dependency_reach``) expose what a GPU is actually good at.
 """
 
 from __future__ import annotations
@@ -25,6 +25,7 @@ from typing import Any
 from .graph.container import UnifiedGraph
 from .graph.dependency_reach import ReachabilityReport, compute_dependency_reach
 from .graph.exposure import exposure_path_rows, materialize_attack_paths, ranked_attack_paths
+from .graph.fix_first import fix_first_view
 
 
 class B200UnsupportedOperationError(NotImplementedError):
@@ -179,6 +180,15 @@ class B200GraphStore:
         if g is None:
             return []
         return materialize_attack_paths(g, exposure_path_rows(g, finding_ids))
+
+    def fix_first_view(self, *, tenant_id: str = "", scan_id: str = "", cve: str = "", package: str = "", agent: str = "", limit: int = 8) -> dict[str, Any]:
+        """The body of ``GET /v1/graph/views/fix-first`` (reference api/routes/graph.py:1110-1166) for the resolved snapshot, ranked on
+        the device; a missing snapshot gives the view of an empty graph, as the route's ``load_graph`` does.  The route keeps its own
+        503 when there is no snapshot at all."""
+        g = self._graph(tenant_id, scan_id)
+        if g is None:
+            g = UnifiedGraph(scan_id=scan_id, tenant_id=tenant_id)
+        return fix_first_view(g, cve=cve, package=package, agent=agent, limit=limit)
 
     def dependency_reach(self, *, tenant_id: str = "", scan_id: str = "") -> ReachabilityReport | None:
         g = self._graph(tenant_id, scan_id)

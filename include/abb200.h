@@ -313,6 +313,20 @@ void abb_paths_result_free(abb_paths_result *r);
 typedef struct abb_rank_result abb_rank_result;
 int abb_paths_rank_host(abb_graph *g, const int32_t *findings, int64_t n_findings, const int32_t *base_id, const uint32_t *risk_rank,
                         int64_t n_base, const int32_t *ncu, const int32_t *ntu, int64_t offset, int64_t limit, abb_rank_result **out);
+
+/* Focused ranking — the fix-first view's cve / package / agent filter (api/routes/graph.py:448-476).  node_focus[n_nodes]
+ * holds ABB_FOCUS_* bits per node (see the table in csrc/paths.cuh); a row matches when every category in `need`
+ * (ABB_FOCUS_CVE | ABB_FOCUS_PACKAGE | ABB_FOCUS_AGENT) is set on one of its hops, ABB_FOCUS_CVE_FINDING counting as CVE on the
+ * finding hop only.  Only the matched rows are sorted (same order as above); the page is taken from them.  total stays the
+ * count of all rows, matched counts the rows that pass.  node_focus == NULL: every row matches (abb_paths_rank_host). */
+#define ABB_FOCUS_CVE 0x1u
+#define ABB_FOCUS_CVE_FINDING 0x2u
+#define ABB_FOCUS_PACKAGE 0x4u
+#define ABB_FOCUS_AGENT 0x8u
+int abb_paths_rank_focus_host(abb_graph *g, const int32_t *findings, int64_t n_findings, const int32_t *base_id, const uint32_t *risk_rank,
+                              int64_t n_base, const int32_t *ncu, const int32_t *ntu, const uint8_t *node_focus, uint32_t need, int64_t offset,
+                              int64_t limit, abb_rank_result **out);
+int64_t abb_rank_result_matched(const abb_rank_result *r);
 int64_t abb_rank_result_total(const abb_rank_result *r);
 int64_t abb_rank_result_count(const abb_rank_result *r);
 const int32_t *abb_rank_result_hops(const abb_rank_result *r);       /* [count*4] */
