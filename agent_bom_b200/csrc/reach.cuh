@@ -12,23 +12,31 @@ namespace abb {
 
 constexpr int ET_PACKAGE = 2;
 
-// one thread per emitted (agent q, package) pair of pass 1
-__global__ void reach_invert_kernel(int64_t nq, const int32_t *agents, const int64_t *q_start, const int32_t *q_count, const int32_t *nodes,
-                                    const int32_t *depth, const int32_t *rank, unsigned long long *keys, int32_t *vals,
+// q_count widened to int64 plus one trailing zero: the input of the exclusive scan that gives every query its output range
+__global__ void reach_qcount_kernel(int64_t nq, const int32_t *q_count, int64_t *out) {
+    const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (i <= nq) out[i] = i < nq ? q_count[i] : 0;
+}
+
+// one thread per emitted (agent q, package) pair of pass 1.
+// A de-duplicated walk points every member of a frontier group at the group's one slice, so the slice at q_start[q] may be
+// shared by several queries: outputs are indexed by qoff (exclusive scan of q_count), not q_start.
+__global__ void reach_invert_kernel(int64_t nq, const int32_t *agents, const int64_t *q_start, const int32_t *q_count, const int64_t *qoff,
+                                    const int32_t *nodes, const int32_t *depth, const int32_t *rank, unsigned long long *keys, int32_t *vals,
                                     unsigned long long *cnt, int32_t *minhop) {
     // a warp per query keeps the slice reads coalesced
     const int lane = threadIdx.x & 31;
     const int64_t warp = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = (static_cast<int64_t>(gridDim.x) * blockDim.x) >> 5;
     for (int64_t q = warp; q < nq; q += nwarps) {
-        const int64_t s = q_start[q];
+        const int64_t s = q_start[q], w = qoff[q];
         const int c = q_count[q];
         const int32_t a = agents[q];
         const unsigned long long ar = static_cast<uint32_t>(rank[a]);
         for (int i = lane; i < c; i += 32) {
             int32_t pkg = nodes[s + i];
-            keys[s + i] = (static_cast<unsigned long long>(static_cast<uint32_t>(pkg)) << 32) | ar;
-            vals[s + i] = a;
+            keys[w + i] = (static_cast<unsigned long long>(static_cast<uint32_t>(pkg)) << 32) | ar;
+            vals[w + i] = a;
             atomicAdd(cnt + pkg, 1ull);
             atomicMin(minhop + pkg, depth[s + i]);
         }

@@ -119,13 +119,16 @@ def test_distances_unbounded_masked(key, dedup):
     """_bfs_distances_along: unbounded depth — on the big seeded graphs this exercises the overflow tiers."""
     og, dg, _, _, _ = graphs_for(key)
     dg.set_dedup(dedup)
-    rng = np.random.default_rng(17)
-    sources = rng.integers(0, og.n_nodes, size=300).astype(np.int32)
-    for mask in (REACH4, 0xFFFFFFFF, LATERAL | REACH4):
-        want = orc.distances_many(og, sources, mask)
-        got = dg.walk(dg.spec_distances(mask), sources)
-        assert_slices_equal(got, want, gpu_aux="depth")
-        np.testing.assert_array_equal(got.maxd, want.maxd)
+    try:
+        rng = np.random.default_rng(17)
+        sources = rng.integers(0, og.n_nodes, size=300).astype(np.int32)
+        for mask in (REACH4, 0xFFFFFFFF, LATERAL | REACH4):
+            want = orc.distances_many(og, sources, mask)
+            got = dg.walk(dg.spec_distances(mask), sources)
+            assert_slices_equal(got, want, gpu_aux="depth")
+            np.testing.assert_array_equal(got.maxd, want.maxd)
+    finally:
+        dg.set_dedup(True)
 
 
 @pytest.mark.parametrize("key", SEEDED + ["estate_150", "estate_dense_40", "kat_probe"])
@@ -269,32 +272,42 @@ def test_bfs_vs_reference_golden(name):
             assert paths == c["paths"]
 
 
+@pytest.mark.parametrize("dedup", [True, False])
 @pytest.mark.parametrize("key", SEEDED[:3] + ALL_FIXTURES)
-def test_dependency_reach(key):
+def test_dependency_reach(key, dedup):
     og, dg, nt, rank, _ = graphs_for(key)
-    agents = np.flatnonzero(nt == 0).astype(np.int32)
-    want = orc.dependency_reach(og, agents, REACH4, VULN_PKG, rank)
-    got = dg.dependency_reach(agents, REACH4, VULN_PKG)
-    for k in ("pkg_ids", "pkg_off", "pkg_agents", "pkg_minhop", "vuln_ids", "vuln_poff", "vuln_pkgs", "vuln_aoff", "vuln_agents", "vuln_minhop"):
-        np.testing.assert_array_equal(got[k], want[k], err_msg=k)
+    dg.set_dedup(dedup)
+    try:
+        agents = np.flatnonzero(nt == 0).astype(np.int32)
+        want = orc.dependency_reach(og, agents, REACH4, VULN_PKG, rank)
+        got = dg.dependency_reach(agents, REACH4, VULN_PKG)
+        for k in ("pkg_ids", "pkg_off", "pkg_agents", "pkg_minhop", "vuln_ids", "vuln_poff", "vuln_pkgs", "vuln_aoff", "vuln_agents", "vuln_minhop"):
+            np.testing.assert_array_equal(got[k], want[k], err_msg=k)
+    finally:
+        dg.set_dedup(True)
 
 
+@pytest.mark.parametrize("dedup", [True, False])
 @pytest.mark.parametrize("key", [SEEDED[2], "mesh_inventory", "estate_dense_40"])
-def test_dependency_reach_device_merge_of_agent_shards(key):
+def test_dependency_reach_device_merge_of_agent_shards(key, dedup):
     """a9 across ranks: per-shard device results merged by the CUDA path of dist.merge_dependency_reach (64-bit key sort on the
     device) == the numpy merge == the unsplit call."""
     from agent_bom_b200.dist import REACH_KEYS, merge_dependency_reach
 
     og, dg, nt, rank, _ = graphs_for(key)
-    agents = np.flatnonzero(nt == 0).astype(np.int32)
-    whole = dg.dependency_reach(agents, REACH4, VULN_PKG)
-    for cuts in ([0, len(agents) // 2, len(agents)], [0, 1, len(agents) // 3, len(agents) // 3, len(agents)]):
-        parts = [dg.dependency_reach(agents[a:b], REACH4, VULN_PKG) for a, b in zip(cuts, cuts[1:])]
-        on_device = merge_dependency_reach(parts, rank, "cuda:0")
-        on_host = merge_dependency_reach(parts, rank)
-        for k in REACH_KEYS:
-            np.testing.assert_array_equal(np.asarray(on_device[k]), np.asarray(whole[k]), err_msg=k)
-            np.testing.assert_array_equal(np.asarray(on_host[k]), np.asarray(whole[k]), err_msg=k)
+    dg.set_dedup(dedup)
+    try:
+        agents = np.flatnonzero(nt == 0).astype(np.int32)
+        whole = dg.dependency_reach(agents, REACH4, VULN_PKG)
+        for cuts in ([0, len(agents) // 2, len(agents)], [0, 1, len(agents) // 3, len(agents) // 3, len(agents)]):
+            parts = [dg.dependency_reach(agents[a:b], REACH4, VULN_PKG) for a, b in zip(cuts, cuts[1:])]
+            on_device = merge_dependency_reach(parts, rank, "cuda:0")
+            on_host = merge_dependency_reach(parts, rank)
+            for k in REACH_KEYS:
+                np.testing.assert_array_equal(np.asarray(on_device[k]), np.asarray(whole[k]), err_msg=k)
+                np.testing.assert_array_equal(np.asarray(on_host[k]), np.asarray(whole[k]), err_msg=k)
+    finally:
+        dg.set_dedup(True)
 
 
 def test_exposure_many_matches_separate_calls():
