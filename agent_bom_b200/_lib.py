@@ -65,6 +65,8 @@ QFLAG_TRUNCATED, QFLAG_NO_ROOT, QFLAG_TARGET_FOUND = 1, 2, 4
 # focus bits of the fix-first ranking (include/abb200.h, table in csrc/paths.cuh)
 FOCUS_CVE, FOCUS_CVE_FINDING, FOCUS_PACKAGE, FOCUS_AGENT = 0x1, 0x2, 0x4, 0x8
 DIR_FORWARD, DIR_REVERSE, DIR_BOTH = 1, 2, 3
+# source-list buckets of the finding context (include/abb200.h, csrc/context.cuh)
+CTX_AGENT, CTX_SERVER, CTX_PACKAGE, CTX_CREDENTIAL, CTX_BUCKETS = 0, 1, 2, 3, 4
 
 #: every symbol include/abb200.h declares (tests assert the .so exports all of them)
 EXPORTS = {
@@ -148,6 +150,22 @@ EXPORTS = {
     "abb_rank_result_row": (vp, [vp]),
     "abb_rank_result_free": (None, [vp]),
     "abb_exposure_host": (C.c_int, [vp, vp, i64, i32, C.POINTER(vp), C.POINTER(vp)]),
+    "abb_finding_context_host": (C.c_int, [vp, i32, vp, i64, C.POINTER(vp)]),
+    "abb_finding_context_result_queries": (i64, [vp]),
+    "abb_finding_context_result_count": (vp, [vp]),
+    "abb_finding_context_result_maxd": (vp, [vp]),
+    "abb_finding_context_result_flags": (vp, [vp]),
+    "abb_finding_context_result_hist_packed": (vp, [vp, vp, vp]),
+    "abb_finding_context_result_hist": (vp, [vp]),
+    "abb_finding_context_result_start": (vp, [vp]),
+    "abb_finding_context_result_bucket_counts": (vp, [vp]),
+    "abb_finding_context_result_total_sources": (i64, [vp]),
+    "abb_finding_context_result_sources": (vp, [vp]),
+    "abb_finding_context_result_h2d_bytes": (i64, [vp]),
+    "abb_finding_context_result_d2h_bytes": (i64, [vp]),
+    "abb_finding_context_result_walk_ms": (C.c_float, [vp]),
+    "abb_finding_context_result_context_ms": (C.c_float, [vp]),
+    "abb_finding_context_result_free": (None, [vp]),
     "abb_dependency_reach_host": (C.c_int, [vp, vp, i64, u32, u32, C.POINTER(vp)]),
     "abb_reach_n_packages": (i64, [vp]),
     "abb_reach_pkg_ids": (vp, [vp]),

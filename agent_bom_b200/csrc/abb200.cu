@@ -23,6 +23,7 @@
 #include "../../include/abb200.h"
 #include "dedup.cuh"
 #include "paths.cuh"
+#include "context.cuh"
 #include "histpack.cuh"
 #include "reach.cuh"
 #include "union.cuh"
@@ -252,6 +253,11 @@ struct abb_graph {
     int64_t paths_n_links = 0, paths_n_template_rows = 0;
     int replicate_grid = 0, rank_keys_grid = 0;   // grids of the row-parallel kernels (row_grid)
     int64_t hint_rows = 0;
+    // finding-context workspace (context.cuh): per-finding bucket counts, totals, start offsets, source lists; the context kernels run on
+    // paths_stream next to the impact walk (cx_staged: the findings are on the device), cx_ev time the count and fill passes
+    DevBuf cx_bcnt, cx_cnt, cx_start, cx_src;
+    cudaEvent_t cx_staged = nullptr;
+    cudaEvent_t cx_ev[4] = {nullptr, nullptr, nullptr, nullptr};
     // owned graph arrays
     std::vector<void *> owned_ptrs;
 };
@@ -273,6 +279,8 @@ static int graph_finish_init(abb_graph *g) {
     CUDA_TRY(cudaEventCreateWithFlags(&g->ev_chunk_walked, cudaEventDisableTiming));
     for (auto &e : g->ev_chunk_copied) CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     for (auto &e : g->ev) CUDA_TRY(cudaEventCreate(&e));
+    CUDA_TRY(cudaEventCreateWithFlags(&g->cx_staged, cudaEventDisableTiming));
+    for (auto &e : g->cx_ev) CUDA_TRY(cudaEventCreate(&e));
     if (int rc = g->ctl.ensure(CTL_WORDS * sizeof(unsigned long long))) return rc;
     const int64_t n = g->v.n;
     g->g_words = (n + 31) / 32 + 1;
@@ -459,6 +467,9 @@ extern "C" void abb_graph_free(abb_graph *g) {
     if (g->ev_chunk_walked) cudaEventDestroy(g->ev_chunk_walked);
     for (auto &e : g->ev_chunk_copied) if (e) cudaEventDestroy(e);
     for (auto &e : g->ev) if (e) cudaEventDestroy(e);
+    if (g->cx_staged) cudaEventDestroy(g->cx_staged);
+    for (auto &e : g->cx_ev) if (e) cudaEventDestroy(e);
+    for (DevBuf *b : {&g->cx_bcnt, &g->cx_cnt, &g->cx_start, &g->cx_src}) b->release();
     for (DevBuf *b : {&g->ctl, &g->ov1, &g->ov2, &g->ov3, &g->ov4, &g->b_gq, &g->b_gpar, &g->b_gdep, &g->g_bitmap, &g->g_queue, &g->g_par, &g->g_dep, &g->x_bitmap, &g->x_queue, &g->x_par, &g->x_dep, &g->dd_sig, &g->dd_ssig, &g->dd_q, &g->dd_sq, &g->dd_head, &g->dd_gid, &g->dd_hp, &g->dd_glen, &g->dd_goff, &g->dd_arena, &g->dd_memoff, &g->dd_memsrc, &g->dd_memstate, &g->dd_indiv, &g->dd_cnt, &g->dd_tmp, &g->dd_lkey, &g->dd_lkey2, &g->dd_lgid, &g->dd_order, &g->dd_gstart, &g->dd_gcount, &g->dd_gmaxd, &g->dd_gflags, &g->dd_ghist, &g->d_histinfo, &g->d_hist_packed, &g->d_nodes_alt, &g->ck_roots, &g->ck_sig, &g->ck_key, &g->ck_key2, &g->ck_idx, &g->ck_order, &g->ck_counts, &g->ck_tmp, &g->ck_qstart, &g->ck_qcount, &g->ck_qmaxd, &g->ck_qflags, &g->ck_qhist, &g->identity_rank, &g->d_roots, &g->d_root_off,
                       &g->d_targets, &g->d_qstart, &g->d_qcount, &g->d_qmaxd, &g->d_qflags, &g->d_qestart, &g->d_qecount, &g->d_qhist, &g->d_nodes,
                       &g->d_parent, &g->d_depth, &g->d_edges, &g->d_totals, &g->p_findings, &g->p_counts, &g->p_off, &g->p_hops, &g->p_rels,
@@ -949,8 +960,10 @@ extern "C" int64_t abb_walk_result_d2h_bytes(const abb_walk_result *r) { return 
 // `direct_nodes`: when the result size is known from the previous call, the walk kernels write the node arena
 // straight into that pinned host block (UVA), so the PCIe transfer of the largest output overlaps the traversal
 // instead of following it; if the estimate turns out too small the walk is re-run into a device arena.
+// `roots_staged`: the caller has already copied the single roots into g->d_roots on g->stream (sized for nq + 1).
 static int walk_device_stage(abb_graph *g, const abb_walk_spec *spec, const int32_t *roots, const int64_t *root_off, const int32_t *targets,
-                             int64_t nq, abb_walk_io *io_out, unsigned long long (&totals)[3], int64_t *h2d, HostBlock *direct_nodes = nullptr) {
+                             int64_t nq, abb_walk_io *io_out, unsigned long long (&totals)[3], int64_t *h2d, HostBlock *direct_nodes = nullptr,
+                             bool roots_staged = false) {
     cudaStream_t st = g->stream;
     const uint32_t fl = spec->flags;
     g->hist_info_valid = false;
@@ -968,7 +981,7 @@ static int walk_device_stage(abb_graph *g, const abb_walk_spec *spec, const int3
     if (fl & ABB_WALK_HIST) if (int rc = g->d_qhist.ensure(q1 * ABB_N_ENTITY_TYPES * 4)) return rc;
     if (int rc = g->d_totals.ensure(3 * sizeof(unsigned long long))) return rc;
     *h2d = 0;
-    if (n_roots) { CUDA_TRY(cudaMemcpyAsync(g->d_roots.p, roots, static_cast<size_t>(n_roots) * 4, cudaMemcpyHostToDevice, st)); *h2d += n_roots * 4; }
+    if (n_roots && !roots_staged) { CUDA_TRY(cudaMemcpyAsync(g->d_roots.p, roots, static_cast<size_t>(n_roots) * 4, cudaMemcpyHostToDevice, st)); *h2d += n_roots * 4; }
     if (root_off) { CUDA_TRY(cudaMemcpyAsync(g->d_root_off.p, root_off, q1 * 8, cudaMemcpyHostToDevice, st)); *h2d += static_cast<int64_t>(q1) * 8; }
     if (fl & ABB_WALK_TARGET) { CUDA_TRY(cudaMemcpyAsync(g->d_targets.p, targets, static_cast<size_t>(nq) * 4, cudaMemcpyHostToDevice, st)); *h2d += nq * 4; }
 
@@ -1041,8 +1054,9 @@ static int walk_device_stage(abb_graph *g, const abb_walk_spec *spec, const int3
 
 // sync == false: the copies go to the graph's copy stream (ordered after everything enqueued so far on the main stream)
 // so that kernels enqueued next on the main stream overlap them; the caller synchronises the copy stream.
+// with_slices == false: only the per-query count / maxd / flags and histograms cross; q_start and the node arena stay on the device.
 static int walk_collect(abb_graph *g, const abb_walk_spec *spec, const abb_walk_io &io, const unsigned long long totals[3], int64_t h2d,
-                        abb_walk_result **out, bool sync, HostBlock *direct_nodes = nullptr) {
+                        abb_walk_result **out, bool sync, HostBlock *direct_nodes = nullptr, bool with_slices = true) {
     cudaStream_t st = g->stream;
     if (!sync) {
         CUDA_TRY(cudaEventRecord(g->ev_copy, g->stream));
@@ -1052,12 +1066,13 @@ static int walk_collect(abb_graph *g, const abb_walk_spec *spec, const abb_walk_
     const uint32_t fl = spec->flags;
     const int64_t nq = io.n_queries;
     abb_walk_result *r = new abb_walk_result();
-    r->nq = nq; r->flags = fl; r->total_nodes = static_cast<int64_t>(totals[0]); r->total_edges = (fl & ABB_WALK_EDGES) ? static_cast<int64_t>(totals[1]) : 0;
+    r->nq = nq; r->flags = fl; r->total_nodes = with_slices ? static_cast<int64_t>(totals[0]) : 0; r->total_edges = (fl & ABB_WALK_EDGES) ? static_cast<int64_t>(totals[1]) : 0;
     r->h2d = h2d;
     const size_t q = static_cast<size_t>(nq), tn = static_cast<size_t>(r->total_nodes), te = static_cast<size_t>(r->total_edges);
     const bool have_nodes = direct_nodes && direct_nodes->p != nullptr;     // already written by the kernels over PCIe
     if (have_nodes) { r->nodes = *direct_nodes; direct_nodes->p = nullptr; direct_nodes->bytes = 0; }
-    bool ok = r->q_start.alloc(q * 8) && r->q_count.alloc(q * 4) && r->q_maxd.alloc(q * 4) && r->q_flags.alloc(q * 4) && (have_nodes || r->nodes.alloc(tn * 4));
+    bool ok = (!with_slices || r->q_start.alloc(q * 8)) && r->q_count.alloc(q * 4) && r->q_maxd.alloc(q * 4) && r->q_flags.alloc(q * 4) &&
+              (have_nodes || !with_slices || r->nodes.alloc(tn * 4));
     if (fl & ABB_WALK_EDGES) ok = ok && r->q_estart.alloc(q * 8) && r->q_ecount.alloc(q * 8) && r->edges.alloc(te * 4);
     const bool pack = (fl & ABB_WALK_HIST) && g->hist_info_valid;
     g->hist_info_valid = false;
@@ -1079,8 +1094,9 @@ static int walk_collect(abb_graph *g, const abb_walk_spec *spec, const abb_walk_
     };
     cudaError_t e = cudaSuccess;
     auto acc = [&](cudaError_t x) { if (e == cudaSuccess) e = x; };
-    acc(d2h(r->q_start, io.q_start, q * 8)); acc(d2h(r->q_count, io.q_count, q * 4)); acc(d2h(r->q_maxd, io.q_maxd, q * 4)); acc(d2h(r->q_flags, io.q_flags, q * 4));
-    if (have_nodes) r->d2h += static_cast<int64_t>((totals[2] ? totals[2] : static_cast<unsigned long long>(tn)) * 4); else acc(d2h(r->nodes, io.nodes, tn * 4));
+    if (with_slices) acc(d2h(r->q_start, io.q_start, q * 8));
+    acc(d2h(r->q_count, io.q_count, q * 4)); acc(d2h(r->q_maxd, io.q_maxd, q * 4)); acc(d2h(r->q_flags, io.q_flags, q * 4));
+    if (have_nodes) r->d2h += static_cast<int64_t>((totals[2] ? totals[2] : static_cast<unsigned long long>(tn)) * 4); else if (with_slices) acc(d2h(r->nodes, io.nodes, tn * 4));
     if (fl & ABB_WALK_EDGES) { acc(d2h(r->q_estart, io.q_estart, q * 8)); acc(d2h(r->q_ecount, io.q_ecount, q * 8)); acc(d2h(r->edges, io.edges, te * 4)); }
     if (pack) {
         if (hc.k) {
@@ -1782,6 +1798,106 @@ extern "C" int abb_exposure_host(abb_graph *g, const int32_t *findings, int64_t 
     }
     if (trace) fprintf(stderr, "[abb] exposure_host: stage+walk %.2f ms, result copies %.2f ms, wait for the path pipeline %.2f ms\n", ms(t0, t1), ms(t1, t2), ms(t2, t3));
     *impact_out = wr; *paths_out = pr;
+    return ABB_OK;
+}
+
+// ------------------------------------------------------------------ finding context (context.cuh)
+struct abb_finding_context_result {
+    int64_t nq = 0, total = 0, h2d = 0, d2h = 0;
+    float walk_ms = -1.f, context_ms = -1.f;
+    abb_walk_result *walk = nullptr;   // count / maxd / flags / histogram of the impact walk; no slices
+    HostBlock start, bcnt, src;
+};
+extern "C" void abb_finding_context_result_free(abb_finding_context_result *r) {
+    if (!r) return;
+    abb_walk_result_free(r->walk);
+    for (HostBlock *b : {&r->start, &r->bcnt, &r->src}) b->release();
+    delete r;
+}
+extern "C" int64_t abb_finding_context_result_queries(const abb_finding_context_result *r) { return r->nq; }
+extern "C" const int32_t *abb_finding_context_result_count(const abb_finding_context_result *r) { return abb_walk_result_count(r->walk); }
+extern "C" const int32_t *abb_finding_context_result_maxd(const abb_finding_context_result *r) { return abb_walk_result_maxd(r->walk); }
+extern "C" const int32_t *abb_finding_context_result_flags(const abb_finding_context_result *r) { return abb_walk_result_flags(r->walk); }
+extern "C" const void *abb_finding_context_result_hist_packed(const abb_finding_context_result *r, uint32_t *columns_mask, int32_t *bytes_per_count) {
+    return abb_walk_result_hist_packed(r->walk, columns_mask, bytes_per_count);
+}
+extern "C" const uint32_t *abb_finding_context_result_hist(const abb_finding_context_result *r) { return abb_walk_result_hist(r->walk); }
+extern "C" const int64_t *abb_finding_context_result_start(const abb_finding_context_result *r) { return r->start.as<int64_t>(); }
+extern "C" const int32_t *abb_finding_context_result_bucket_counts(const abb_finding_context_result *r) { return r->bcnt.as<int32_t>(); }
+extern "C" int64_t abb_finding_context_result_total_sources(const abb_finding_context_result *r) { return r->total; }
+extern "C" const int32_t *abb_finding_context_result_sources(const abb_finding_context_result *r) { return r->src.as<int32_t>(); }
+extern "C" int64_t abb_finding_context_result_h2d_bytes(const abb_finding_context_result *r) { return r->h2d; }
+extern "C" int64_t abb_finding_context_result_d2h_bytes(const abb_finding_context_result *r) { return r->d2h; }
+extern "C" float abb_finding_context_result_walk_ms(const abb_finding_context_result *r) { return r->walk_ms; }
+extern "C" float abb_finding_context_result_context_ms(const abb_finding_context_result *r) { return r->context_ms; }
+
+// The findings are staged once.  The context count pass and its scan run on paths_stream while this thread runs the impact walk on the
+// main stream into a device arena (walk_device_stage without a host block); then the fill pass runs on paths_stream while the walk's
+// per-finding arrays (not its slices) are copied back on the main stream.
+extern "C" int abb_finding_context_host(abb_graph *g, int32_t max_depth, const int32_t *findings, int64_t n_findings, abb_finding_context_result **out) {
+    NvtxRange nvtx_("abb_finding_context_host");
+    if (!g || !out || n_findings < 0 || (n_findings && !findings)) return fail(ABB_ERR_ARG, "bad arguments");
+    if (n_findings >= (1ll << 31) - 2) return fail(ABB_ERR_ARG, "too many findings in one batch");
+    DeviceGuard dg(g->device);
+    std::lock_guard<std::mutex> lk(g->mu);
+    cudaStream_t st = g->stream, cs = g->paths_stream;
+    const int64_t nq = n_findings;
+    const size_t q = static_cast<size_t>(nq), q1 = q + 1;
+    auto drain = [&]() { cudaStreamSynchronize(st); cudaStreamSynchronize(cs); };
+    int rc = ABB_OK;
+#define ENS(buf, bytes) if (!rc) rc = g->buf.ensure(static_cast<size_t>(bytes))
+    ENS(d_roots, q1 * 4); ENS(cx_bcnt, q1 * CTX_BUCKETS * 4); ENS(cx_cnt, q1 * 8); ENS(cx_start, q1 * 8);
+    if (rc) return rc;
+    std::unique_ptr<abb_finding_context_result, void (*)(abb_finding_context_result *)> r(new abb_finding_context_result(), abb_finding_context_result_free);
+    r->nq = nq;
+    if (nq) CUDA_TRY(cudaMemcpyAsync(g->d_roots.p, findings, q * 4, cudaMemcpyHostToDevice, st));
+    r->h2d = nq * 4;
+    CUDA_TRY(cudaEventRecord(g->cx_staged, st));
+    CUDA_TRY(cudaStreamWaitEvent(cs, g->cx_staged, 0));
+    // count pass + scan, next to the walk
+    CtxArgs A{};
+    A.g = g->v; A.findings = g->d_roots.as<int32_t>(); A.n = nq;
+    A.bcnt = g->cx_bcnt.as<int32_t>(); A.cnt = g->cx_cnt.as<int64_t>(); A.start = g->cx_start.as<int64_t>();
+    const unsigned grid = warp_grid(g, (nq + 31) / 32);
+    CUDA_TRY(cudaEventRecord(g->cx_ev[0], cs));
+    CUDA_TRY(cudaMemsetAsync(A.cnt, 0, q1 * 8, cs));
+    if (nq) { context_kernel<false><<<grid, 256, 0, cs>>>(A); g_launches++; }
+    if ((rc = scan_i64(g, A.cnt, g->cx_start.as<int64_t>(), nq + 1, cs))) { drain(); return rc; }
+    CUDA_TRY(cudaEventRecord(g->cx_ev[1], cs));
+    // the impact walk, unchanged, into the device arena
+    const abb_walk_spec spec = abb_spec_impact_of(max_depth);
+    abb_walk_io io{}; unsigned long long totals[3] = {0, 0, 0}; int64_t wh2d = 0;
+    g->last_host_chunks = 1;
+    if ((rc = walk_device_stage(g, &spec, findings, nullptr, nullptr, nq, &io, totals, &wh2d, nullptr, true))) { drain(); return rc; }
+    int64_t total = 0;
+    CUDA_TRY(cudaMemcpyAsync(&total, g->cx_start.as<int64_t>() + nq, 8, cudaMemcpyDeviceToHost, cs));
+    CUDA_TRY(cudaStreamSynchronize(cs));
+    r->total = total;
+    ENS(cx_src, (total + 1) * 4);
+#undef ENS
+    if (rc) { drain(); return rc; }
+    if (!(r->start.alloc(q * 8) && r->bcnt.alloc(q * CTX_BUCKETS * 4) && r->src.alloc(static_cast<size_t>(total) * 4))) {
+        drain(); return fail(ABB_ERR_NOMEM, "pinned host allocation failed");
+    }
+    // fill pass and its copies on paths_stream, the walk's per-finding arrays on the main stream
+    A.src = g->cx_src.as<int32_t>();
+    CUDA_TRY(cudaEventRecord(g->cx_ev[2], cs));
+    if (nq) { context_kernel<true><<<grid, 256, 0, cs>>>(A); g_launches++; }
+    CUDA_TRY(cudaEventRecord(g->cx_ev[3], cs));
+    cudaError_t e = cudaGetLastError();
+    auto d2h = [&](HostBlock &dst, const void *src, size_t bytes) {
+        r->d2h += static_cast<int64_t>(bytes);
+        if (e == cudaSuccess && bytes) e = cudaMemcpyAsync(dst.p, src, bytes, cudaMemcpyDeviceToHost, cs);
+    };
+    d2h(r->start, g->cx_start.p, q * 8); d2h(r->bcnt, g->cx_bcnt.p, q * CTX_BUCKETS * 4); d2h(r->src, g->cx_src.p, static_cast<size_t>(total) * 4);
+    if (e != cudaSuccess) { drain(); return fail(ABB_ERR_CUDA, "finding context failed: %s", cudaGetErrorString(e)); }
+    if ((rc = walk_collect(g, &spec, io, totals, wh2d, &r->walk, true, nullptr, false))) { drain(); return rc; }
+    if ((e = cudaStreamSynchronize(cs)) != cudaSuccess) { drain(); return fail(ABB_ERR_CUDA, "finding context failed: %s", cudaGetErrorString(e)); }
+    r->d2h += r->walk->d2h;
+    float a = 0.f, b = 0.f;
+    if (cudaEventElapsedTime(&a, g->ev[0], g->ev[1]) == cudaSuccess) r->walk_ms = a;
+    if (cudaEventElapsedTime(&a, g->cx_ev[0], g->cx_ev[1]) == cudaSuccess && cudaEventElapsedTime(&b, g->cx_ev[2], g->cx_ev[3]) == cudaSuccess) r->context_ms = a + b;
+    *out = r.release();
     return ABB_OK;
 }
 

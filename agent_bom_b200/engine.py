@@ -114,6 +114,39 @@ class WalkResult:
 
 
 @dataclass
+class FindingContext:
+    """What the OCSF export's ``graph_context`` needs per finding q, from ``DeviceGraph.finding_context``: the impact walk's
+    ``count`` / ``maxd`` / ``flags`` / type histogram (no node slices), and the finding's in-neighbours of the four listed kinds —
+    ``sources(q, bucket)`` with ``bucket`` one of ``_lib.CTX_AGENT`` / ``CTX_SERVER`` / ``CTX_PACKAGE`` / ``CTX_CREDENTIAL``, in
+    ``reverse_adjacency`` order with duplicates kept."""
+
+    count: np.ndarray
+    maxd: np.ndarray
+    flags: np.ndarray
+    start: np.ndarray              # int64 [n] first source of finding q
+    bucket_counts: np.ndarray      # int32 [n, CTX_BUCKETS]
+    source_nodes: np.ndarray       # int32, bucket-major within a finding
+    h2d_bytes: int = 0
+    d2h_bytes: int = 0
+    kernel_ms: float = 0.0         # the impact walk's kernels
+    context_ms: float = 0.0        # the context kernels (count + fill passes; they overlap the walk on another stream)
+    hist_packed: np.ndarray | None = None
+    hist_cols: np.ndarray | None = None
+    _hist: np.ndarray | None = None
+
+    hist = WalkResult.hist
+    hist_dict = WalkResult.hist_dict
+
+    def __len__(self) -> int:
+        return int(self.count.shape[0])
+
+    def sources(self, q: int, bucket: int) -> np.ndarray:
+        bc = self.bucket_counts[q]
+        s = int(self.start[q]) + int(bc[:bucket].sum())
+        return self.source_nodes[s: s + int(bc[bucket])]
+
+
+@dataclass
 class PathRows:
     """Exposure-path rows in the reference's emission order (before risk ranking)."""
 
@@ -398,6 +431,38 @@ class DeviceGraph:
             lib.abb_walk_result_free(wres)
             lib.abb_paths_result_free(pres)
         return w, p
+
+    def finding_context(self, findings, max_depth: int = 4) -> FindingContext:
+        """Per finding: ``impact_of``'s count, depth, flags and type histogram plus its typed in-neighbour lists
+        (``abb_finding_context_host``).  The walk's node slices stay on the device."""
+        lib = _lib.load()
+        f = _i32(findings)
+        nq = int(f.shape[0])
+        res = _vp()
+        with self._use() as h:
+            _lib.check(lib.abb_finding_context_host(h, int(max_depth), f.ctypes.data, nq, C.byref(res)))
+        try:
+            total = int(lib.abb_finding_context_result_total_sources(res))
+            out = FindingContext(
+                count=_view(lib.abb_finding_context_result_count(res), nq, np.int32), maxd=_view(lib.abb_finding_context_result_maxd(res), nq, np.int32),
+                flags=_view(lib.abb_finding_context_result_flags(res), nq, np.int32), start=_view(lib.abb_finding_context_result_start(res), nq, np.int64),
+                bucket_counts=_view(lib.abb_finding_context_result_bucket_counts(res), nq * _lib.CTX_BUCKETS, np.int32).reshape(nq, _lib.CTX_BUCKETS),
+                source_nodes=_view(lib.abb_finding_context_result_sources(res), total, np.int32),
+                h2d_bytes=int(lib.abb_finding_context_result_h2d_bytes(res)), d2h_bytes=int(lib.abb_finding_context_result_d2h_bytes(res)),
+                kernel_ms=float(lib.abb_finding_context_result_walk_ms(res)), context_ms=float(lib.abb_finding_context_result_context_ms(res)),
+            )
+            mask, width = C.c_uint32(0), C.c_int32(0)
+            packed = lib.abb_finding_context_result_hist_packed(res, C.byref(mask), C.byref(width))
+            if packed:
+                cols = np.array([t for t in range(N_ENTITY_TYPES) if mask.value >> t & 1], dtype=np.int64)
+                dt = np.uint16 if width.value == 2 else np.uint32
+                out.hist_cols = cols
+                out.hist_packed = (_view(packed, nq * len(cols), dt) if len(cols) else np.zeros(0, dt)).reshape(nq, len(cols))
+            else:
+                out.hist = _view(lib.abb_finding_context_result_hist(res), nq * N_ENTITY_TYPES, np.uint32).reshape(nq, N_ENTITY_TYPES)
+            return out
+        finally:
+            lib.abb_finding_context_result_free(res)
 
     def rank_exposure_paths(self, findings, base_id, risk_rank, ncu, ntu, offset: int = 0, limit: int = 100):
         """Page [offset, offset+limit) of the exposure-path rows in the reference's ranking order; returns (PathRows-like, risk_rank, total)."""

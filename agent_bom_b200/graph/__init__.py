@@ -13,6 +13,7 @@ from .envelope import EdgeIndex, exposure_path_for_attack_path, mcp_exposure_pat
 from .fix_first import fix_first_view
 from .exposure import derived_attack_paths, exposure_path_rows, materialize_attack_paths, node_risk_100, ranked_attack_paths
 from .model import AttackPath, UnifiedEdge, UnifiedNode
+from .ocsf import iter_ocsf_events, ocsf_event
 from .snapshot import SnapshotGraph, load_snapshot
 from .schema import FINDING_ENTITY_TYPES, SEVERITY_RANK, EntityType, NodeStatus, RelationshipType
 
@@ -20,5 +21,5 @@ __all__ = [
     "AttackPath", "EntityType", "FINDING_ENTITY_TYPES", "NodeStatus", "PackageReachability", "ReachabilityReport", "RelationshipType", "SEVERITY_RANK", "SnapshotGraph", "load_snapshot",
     "UnifiedEdge", "UnifiedGraph", "UnifiedNode", "VulnerabilityReachability", "build_unified_graph_from_report", "compute_dependency_reach", "derived_attack_paths", "exposure_path_rows",
     "materialize_attack_paths", "node_risk_100", "ranked_attack_paths", "EdgeIndex", "exposure_path_for_attack_path", "mcp_exposure_path_payload",
-    "serialize_attack_path", "serialize_attack_paths", "fix_first_view",
+    "serialize_attack_path", "serialize_attack_paths", "fix_first_view", "iter_ocsf_events", "ocsf_event",
 ]

@@ -363,6 +363,17 @@ class UnifiedGraph:
         sample = np.arange(min(50, c.n_real), dtype=np.int32)
         return rank_bottlenecks(c, self.device_graph.bottleneck_scores(sample), top_n)
 
+    # ── OCSF export (reference container.py:628-654) ────────────────────
+    def iter_ocsf_events(self, product_version: str = "0.0.0", *, enrich_neighbors: bool = True, batch_size: int = 65536):
+        """Finding nodes as OCSF events, in ``nodes`` order; with ``enrich_neighbors`` each carries its ``graph_context``
+        (typed in-neighbours, blast radius and its type histogram), computed on the device one batch of findings at a time."""
+        from .ocsf import iter_ocsf_events
+
+        return iter_ocsf_events(self, product_version, enrich_neighbors=enrich_neighbors, batch_size=batch_size)
+
+    def to_ocsf_events(self, product_version: str = "0.0.0", *, enrich_neighbors: bool = True) -> list[dict[str, Any]]:
+        return list(self.iter_ocsf_events(product_version, enrich_neighbors=enrich_neighbors))
+
     # ── serialisation ───────────────────────────────────────────────────
     def to_dict(self) -> dict[str, Any]:
         def nd(n):

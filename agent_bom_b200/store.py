@@ -14,7 +14,7 @@ Conventions kept: keyword-only arguments; a missing snapshot / node yields
 ``None`` / ``([], set())`` / an empty graph, never an exception; methods are
 thread-safe (REST calls arrive on worker threads via ``asyncio.to_thread``).
 Batched extensions (``impact_of_many``, ``exposure_paths_many``,
-``fix_first_view``, ``dependency_reach``) expose what a GPU is actually good at.
+``fix_first_view``, ``ocsf_events``, ``dependency_reach``) expose what a GPU is actually good at.
 """
 
 from __future__ import annotations
@@ -26,6 +26,7 @@ from .graph.container import UnifiedGraph
 from .graph.dependency_reach import ReachabilityReport, compute_dependency_reach
 from .graph.exposure import exposure_path_rows, materialize_attack_paths, ranked_attack_paths
 from .graph.fix_first import fix_first_view
+from .graph.ocsf import iter_ocsf_events
 
 
 class B200UnsupportedOperationError(NotImplementedError):
@@ -189,6 +190,15 @@ class B200GraphStore:
         if g is None:
             g = UnifiedGraph(scan_id=scan_id, tenant_id=tenant_id)
         return fix_first_view(g, cve=cve, package=package, agent=agent, limit=limit)
+
+    def ocsf_events(self, *, tenant_id: str = "", scan_id: str = "", product_version: str = "0.0.0", enrich_neighbors: bool = True, offset: int = 0,
+                    limit: int | None = None) -> list[dict[str, Any]]:
+        """Page [offset, offset+limit) of the snapshot's OCSF finding events (``UnifiedGraph.to_ocsf_events`` order; ``limit=None``:
+        to the end), computed only for that page; ``[]`` for a missing snapshot."""
+        g = self._graph(tenant_id, scan_id)
+        if g is None:
+            return []
+        return list(iter_ocsf_events(g, product_version, enrich_neighbors=enrich_neighbors, offset=offset, limit=limit))
 
     def dependency_reach(self, *, tenant_id: str = "", scan_id: str = "") -> ReachabilityReport | None:
         g = self._graph(tenant_id, scan_id)

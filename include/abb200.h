@@ -347,6 +347,48 @@ int abb_exposure_host(abb_graph *g, const int32_t *findings, int64_t n_findings,
                       abb_walk_result **impact_out, abb_paths_result **paths_out);
 
 /* ------------------------------------------------------------------------
+ * Finding context — the graph_context block of UnifiedGraph.to_ocsf_events
+ * (graph/container.py:628-654) for a batch of findings:
+ *   - the finding's in-neighbours (sources_of: reverse_adjacency[f] in list
+ *     order, reversed twins of bidirectional edges included, duplicates kept)
+ *     whose entity type is agent / server / package / credential, one list per
+ *     ABB_CTX_* bucket; ghosts and every other kind are not listed;
+ *   - impact_of(f, max_depth)'s affected_count, max depth, flags and entity-type
+ *     histogram (the impact walk, unchanged).
+ * The walk's node slices stay in device memory: they never cross PCIe, whatever
+ * the zero_copy / chunks options say.  What comes back, per finding q:
+ * count / maxd / flags (int32), the histogram (packed as abb_walk_result_hist_packed
+ * describes, or dense), start (int64) and bucket counts (int32 [n*ABB_CTX_BUCKETS]);
+ * sources[start[q] ..] holds bucket 0's sources, then bucket 1's, ... in row order.
+ * An invalid or ghost finding index has empty lists (and the walk's NO_ROOT flag).
+ * ---------------------------------------------------------------------- */
+#define ABB_CTX_AGENT 0
+#define ABB_CTX_SERVER 1
+#define ABB_CTX_PACKAGE 2
+#define ABB_CTX_CREDENTIAL 3
+#define ABB_CTX_BUCKETS 4
+#define ABB_CTX_NONE 255
+typedef struct abb_finding_context_result abb_finding_context_result;
+int abb_finding_context_host(abb_graph *g, int32_t max_depth, const int32_t *findings, int64_t n_findings, abb_finding_context_result **out);
+int64_t abb_finding_context_result_queries(const abb_finding_context_result *r);
+const int32_t *abb_finding_context_result_count(const abb_finding_context_result *r);
+const int32_t *abb_finding_context_result_maxd(const abb_finding_context_result *r);
+const int32_t *abb_finding_context_result_flags(const abb_finding_context_result *r);
+/* packed histogram (same contract as abb_walk_result_hist_packed); NULL when the dense table was shipped */
+const void *abb_finding_context_result_hist_packed(const abb_finding_context_result *r, uint32_t *columns_mask, int32_t *bytes_per_count);
+const uint32_t *abb_finding_context_result_hist(const abb_finding_context_result *r);     /* dense [n*ABB_N_ENTITY_TYPES] */
+const int64_t *abb_finding_context_result_start(const abb_finding_context_result *r);     /* [n] */
+const int32_t *abb_finding_context_result_bucket_counts(const abb_finding_context_result *r); /* [n*ABB_CTX_BUCKETS] */
+int64_t abb_finding_context_result_total_sources(const abb_finding_context_result *r);
+const int32_t *abb_finding_context_result_sources(const abb_finding_context_result *r);   /* [total_sources] */
+int64_t abb_finding_context_result_h2d_bytes(const abb_finding_context_result *r);
+int64_t abb_finding_context_result_d2h_bytes(const abb_finding_context_result *r);
+/* device time of the impact walk and of the context kernels (CUDA events; the two run on different streams and overlap) */
+float abb_finding_context_result_walk_ms(const abb_finding_context_result *r);
+float abb_finding_context_result_context_ms(const abb_finding_context_result *r);
+void abb_finding_context_result_free(abb_finding_context_result *r);
+
+/* ------------------------------------------------------------------------
  * compute_dependency_reach — graph/dependency_reach.py:109-220.
  * Pass 1: walk from every agent along rel_mask (unbounded depth), keeping
  * package nodes and hop counts.  Pass 2 (device sort/segment): per package the
