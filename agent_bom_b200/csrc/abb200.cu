@@ -125,16 +125,31 @@ constexpr int CTL_FATAL = 4 * 4 + 2;  // last tier's fatal flag inside a set
 constexpr int CTL_ROUTE = 24;         // {heavy hand-offs routed to the big block tier, to the warp tier} inside a set
 
 // ------------------------------------------------------------------ device buffers
+// The one owner of device memory: freed by its destructor, which must run while the buffer's device is current (scoped
+// buffers are declared after the call's DeviceGuard; abb_graph_free deletes the graph under one).
 struct DevBuf {
     void *p = nullptr; size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(DevBuf &&o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+    DevBuf &operator=(DevBuf &&o) noexcept { if (this != &o) { release(); std::swap(p, o.p); std::swap(cap, o.cap); } return *this; }
+    ~DevBuf() { release(); }
+    // workspace reused across calls: grows with slack, old contents discarded
     int ensure(size_t bytes) {
         if (bytes <= cap) return ABB_OK;
-        if (p) cudaFree(p);
-        p = nullptr; cap = 0;
+        release();
         size_t want = bytes + bytes / 4 + 256;
         cudaError_t e = cudaMalloc(&p, want);
         if (e != cudaSuccess) { e = cudaMalloc(&p, bytes); want = bytes; }
         if (e != cudaSuccess) return fail(ABB_ERR_NOMEM, "cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e));
+        cap = want;
+        return ABB_OK;
+    }
+    // exact size: scratch that lives for one call (the ranking pass's R x 8 B keys leave no room for slack) and graph arrays
+    int alloc(size_t bytes) {
+        release();
+        const size_t want = bytes ? bytes : 16;
+        cudaError_t e = cudaMalloc(&p, want);
+        if (e != cudaSuccess) return fail(ABB_ERR_NOMEM, "cudaMalloc(%zu): %s", bytes, cudaGetErrorString(e));
         cap = want;
         return ABB_OK;
     }
@@ -174,9 +189,14 @@ struct PinnedPool {
 };
 static PinnedPool g_pinned;
 
+// a pinned block of g_pinned, returned to the pool by its destructor
 struct HostBlock {
     void *p = nullptr; size_t bytes = 0;
-    bool alloc(size_t n) { p = g_pinned.get(n, &bytes); return p != nullptr; }
+    HostBlock() = default;
+    HostBlock(HostBlock &&o) noexcept : p(o.p), bytes(o.bytes) { o.p = nullptr; o.bytes = 0; }
+    HostBlock &operator=(HostBlock &&o) noexcept { if (this != &o) { release(); std::swap(p, o.p); std::swap(bytes, o.bytes); } return *this; }
+    ~HostBlock() { release(); }
+    bool alloc(size_t n) { release(); p = g_pinned.get(n, &bytes); return p != nullptr; }
     void release() { g_pinned.put(p, bytes); p = nullptr; bytes = 0; }
     template <class T> T *as() const { return static_cast<T *>(p); }
 };
@@ -184,7 +204,6 @@ struct HostBlock {
 // ------------------------------------------------------------------ graph handle
 struct abb_graph {
     int device = 0;
-    bool owned = false;
     GraphView v{};
     int64_t bytes = 0;
     int sm_count = 132;               // H100 SXM; set from the device in graph_finish_init
@@ -245,7 +264,7 @@ struct abb_graph {
     DevBuf srv_cred, srv_tool, srv_roff, srv_row, srv_rel;
     bool srv_table_ready = false;
     // paths staging
-    DevBuf p_findings, p_counts, p_off, p_hops, p_rels, p_ncred, p_ntool, p_scan_tmp;
+    DevBuf p_findings, p_off, p_scan_tmp;
     // exposure-path pipeline workspace (links, templates)
     DevBuf pl_cnt, pl_off, pl_vs, pl_rel, pl_f, pl_rows, pl_roff, pl_toff, pl_need, pl_ulist, pl_nu, pt_cnt, pt_off, pt_off_node, pt_cnt_node, pt_row, pt_rel;
     PathsArgs paths_args{};
@@ -258,8 +277,15 @@ struct abb_graph {
     DevBuf cx_bcnt, cx_cnt, cx_start, cx_src;
     cudaEvent_t cx_staged = nullptr;
     cudaEvent_t cx_ev[4] = {nullptr, nullptr, nullptr, nullptr};
-    // owned graph arrays
-    std::vector<void *> owned_ptrs;
+    // graph arrays of an uploaded graph (an adopted graph's belong to the caller)
+    std::vector<DevBuf> owned_arrays;
+
+    // Runs with the graph's device current (abb_graph_free); the DevBuf members free themselves after it.
+    ~abb_graph() {
+        for (cudaStream_t s : {stream, copy_stream, paths_stream}) if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); }
+        for (cudaEvent_t e : {ev_copy, ev_chunk_walked, ev_chunk_copied[0], ev_chunk_copied[1], ev[0], ev[1], ev[2], ev[3], cx_staged, cx_ev[0], cx_ev[1], cx_ev[2], cx_ev[3]})
+            if (e) cudaEventDestroy(e);
+    }
 };
 
 struct DeviceGuard {
@@ -352,18 +378,15 @@ extern "C" int abb_graph_upload(int device, const abb_csr *host, abb_graph **out
     if (abb_device_count() <= device || device < 0) return fail(ABB_ERR_CUDA, "no CUDA device %d (this library has no CPU fallback)", device);
     DeviceGuard dg(device);
     abb_graph *g = new abb_graph();
-    g->device = device; g->owned = true;
+    g->device = device;
     abb_csr d = *host;
     const size_t n1 = static_cast<size_t>(host->n_nodes) + 1, m = static_cast<size_t>(host->n_entries);
     auto up = [&](const void *src, size_t bytes, const void **dstp) -> int {
-        void *p = nullptr;
-        size_t alloc = bytes ? bytes : 16;
-        cudaError_t e = cudaMalloc(&p, alloc);
-        if (e != cudaSuccess) return fail(ABB_ERR_NOMEM, "cudaMalloc(%zu): %s", alloc, cudaGetErrorString(e));
-        g->owned_ptrs.push_back(p);
-        if (bytes) { e = cudaMemcpy(p, src, bytes, cudaMemcpyHostToDevice); if (e != cudaSuccess) return fail(ABB_ERR_CUDA, "H2D: %s", cudaGetErrorString(e)); }
+        DevBuf &b = g->owned_arrays.emplace_back();
+        if (int rc = b.alloc(bytes)) return rc;
+        if (bytes) { cudaError_t e = cudaMemcpy(b.p, src, bytes, cudaMemcpyHostToDevice); if (e != cudaSuccess) return fail(ABB_ERR_CUDA, "H2D: %s", cudaGetErrorString(e)); }
         g->bytes += static_cast<int64_t>(bytes);
-        *dstp = p;
+        *dstp = b.p;
         return ABB_OK;
     };
     int rc = ABB_OK;
@@ -385,7 +408,7 @@ extern "C" int abb_graph_adopt(int device, const abb_csr *dev, abb_graph **out) 
     if (abb_device_count() <= device || device < 0) return fail(ABB_ERR_CUDA, "no CUDA device %d (this library has no CPU fallback)", device);
     DeviceGuard dg(device);
     abb_graph *g = new abb_graph();
-    g->device = device; g->owned = false;
+    g->device = device;
     view_from_csr(g->v, dev);
     g->bytes = (static_cast<int64_t>(dev->n_nodes) + 1) * 8 + dev->n_entries * 18 + dev->n_nodes * 5;
     int rc = graph_finish_init(g);
@@ -460,22 +483,6 @@ extern "C" void abb_graph_free(abb_graph *g) {
     if (!g) return;
     DeviceGuard dg(g->device);
     { std::lock_guard<std::mutex> lk(g->mu); }      // a host-API call still inside the library finishes before the teardown starts
-    if (g->stream) { cudaStreamSynchronize(g->stream); cudaStreamDestroy(g->stream); }
-    if (g->copy_stream) { cudaStreamSynchronize(g->copy_stream); cudaStreamDestroy(g->copy_stream); }
-    if (g->paths_stream) { cudaStreamSynchronize(g->paths_stream); cudaStreamDestroy(g->paths_stream); }
-    if (g->ev_copy) cudaEventDestroy(g->ev_copy);
-    if (g->ev_chunk_walked) cudaEventDestroy(g->ev_chunk_walked);
-    for (auto &e : g->ev_chunk_copied) if (e) cudaEventDestroy(e);
-    for (auto &e : g->ev) if (e) cudaEventDestroy(e);
-    if (g->cx_staged) cudaEventDestroy(g->cx_staged);
-    for (auto &e : g->cx_ev) if (e) cudaEventDestroy(e);
-    for (DevBuf *b : {&g->cx_bcnt, &g->cx_cnt, &g->cx_start, &g->cx_src}) b->release();
-    for (DevBuf *b : {&g->ctl, &g->ov1, &g->ov2, &g->ov3, &g->ov4, &g->b_gq, &g->b_gpar, &g->b_gdep, &g->g_bitmap, &g->g_queue, &g->g_par, &g->g_dep, &g->x_bitmap, &g->x_queue, &g->x_par, &g->x_dep, &g->dd_sig, &g->dd_ssig, &g->dd_q, &g->dd_sq, &g->dd_head, &g->dd_gid, &g->dd_hp, &g->dd_glen, &g->dd_goff, &g->dd_arena, &g->dd_memoff, &g->dd_memsrc, &g->dd_memstate, &g->dd_indiv, &g->dd_cnt, &g->dd_tmp, &g->dd_lkey, &g->dd_lkey2, &g->dd_lgid, &g->dd_order, &g->dd_gstart, &g->dd_gcount, &g->dd_gmaxd, &g->dd_gflags, &g->dd_ghist, &g->d_histinfo, &g->d_hist_packed, &g->d_nodes_alt, &g->ck_roots, &g->ck_sig, &g->ck_key, &g->ck_key2, &g->ck_idx, &g->ck_order, &g->ck_counts, &g->ck_tmp, &g->ck_qstart, &g->ck_qcount, &g->ck_qmaxd, &g->ck_qflags, &g->ck_qhist, &g->identity_rank, &g->d_roots, &g->d_root_off,
-                      &g->d_targets, &g->d_qstart, &g->d_qcount, &g->d_qmaxd, &g->d_qflags, &g->d_qestart, &g->d_qecount, &g->d_qhist, &g->d_nodes,
-                      &g->d_parent, &g->d_depth, &g->d_edges, &g->d_totals, &g->p_findings, &g->p_counts, &g->p_off, &g->p_hops, &g->p_rels,
-                      &g->p_ncred, &g->p_ntool, &g->p_scan_tmp, &g->srv_cred, &g->srv_tool, &g->pl_cnt, &g->pl_off, &g->pl_vs, &g->pl_rel, &g->pl_rows, &g->pl_roff, &g->pl_toff, &g->pl_need, &g->pl_ulist, &g->pl_nu, &g->pt_cnt, &g->pt_off, &g->pt_off_node, &g->pt_cnt_node, &g->pt_row, &g->pt_rel})
-        b->release();
-    if (g->owned) for (void *p : g->owned_ptrs) cudaFree(p);
     delete g;
 }
 
@@ -893,12 +900,7 @@ struct abb_walk_result {
     std::mutex mu;
 };
 
-extern "C" void abb_walk_result_free(abb_walk_result *r) {
-    if (!r) return;
-    for (HostBlock *b : {&r->q_start, &r->q_count, &r->q_maxd, &r->q_flags, &r->q_estart, &r->q_ecount, &r->q_hist, &r->q_hist_packed, &r->nodes, &r->parent, &r->depth, &r->edges})
-        b->release();
-    delete r;
-}
+extern "C" void abb_walk_result_free(abb_walk_result *r) { delete r; }
 extern "C" int64_t abb_walk_result_queries(const abb_walk_result *r) { return r->nq; }
 extern "C" int64_t abb_walk_result_total_nodes(const abb_walk_result *r) { return r->total_nodes; }
 extern "C" int64_t abb_walk_result_total_edges(const abb_walk_result *r) { return r->total_edges; }
@@ -1065,12 +1067,12 @@ static int walk_collect(abb_graph *g, const abb_walk_spec *spec, const abb_walk_
     }
     const uint32_t fl = spec->flags;
     const int64_t nq = io.n_queries;
-    abb_walk_result *r = new abb_walk_result();
+    std::unique_ptr<abb_walk_result> r(new abb_walk_result());
     r->nq = nq; r->flags = fl; r->total_nodes = with_slices ? static_cast<int64_t>(totals[0]) : 0; r->total_edges = (fl & ABB_WALK_EDGES) ? static_cast<int64_t>(totals[1]) : 0;
     r->h2d = h2d;
     const size_t q = static_cast<size_t>(nq), tn = static_cast<size_t>(r->total_nodes), te = static_cast<size_t>(r->total_edges);
     const bool have_nodes = direct_nodes && direct_nodes->p != nullptr;     // already written by the kernels over PCIe
-    if (have_nodes) { r->nodes = *direct_nodes; direct_nodes->p = nullptr; direct_nodes->bytes = 0; }
+    if (have_nodes) r->nodes = std::move(*direct_nodes);
     bool ok = (!with_slices || r->q_start.alloc(q * 8)) && r->q_count.alloc(q * 4) && r->q_maxd.alloc(q * 4) && r->q_flags.alloc(q * 4) &&
               (have_nodes || !with_slices || r->nodes.alloc(tn * 4));
     if (fl & ABB_WALK_EDGES) ok = ok && r->q_estart.alloc(q * 8) && r->q_ecount.alloc(q * 8) && r->edges.alloc(te * 4);
@@ -1087,7 +1089,7 @@ static int walk_collect(abb_graph *g, const abb_walk_spec *spec, const abb_walk_
     } else if (fl & ABB_WALK_HIST) ok = ok && r->q_hist.alloc(q * ABB_N_ENTITY_TYPES * 4);
     if (fl & ABB_WALK_PARENTS) ok = ok && r->parent.alloc(tn * 4);
     if (fl & ABB_WALK_DEPTHS) ok = ok && r->depth.alloc(tn * 4);
-    if (!ok) { abb_walk_result_free(r); return fail(ABB_ERR_NOMEM, "pinned host allocation failed"); }
+    if (!ok) return fail(ABB_ERR_NOMEM, "pinned host allocation failed");
     auto d2h = [&](HostBlock &dst, const void *src, size_t bytes) -> cudaError_t {
         r->d2h += static_cast<int64_t>(bytes);
         return bytes ? cudaMemcpyAsync(dst.p, src, bytes, cudaMemcpyDeviceToHost, st) : cudaSuccess;
@@ -1101,7 +1103,7 @@ static int walk_collect(abb_graph *g, const abb_walk_spec *spec, const abb_walk_
     if (pack) {
         if (hc.k) {
             const size_t pbytes = q * hc.k * r->hist_width;
-            if (int rc = g->d_hist_packed.ensure(pbytes)) { abb_walk_result_free(r); return rc; }
+            if (int rc = g->d_hist_packed.ensure(pbytes)) return rc;
             const unsigned grid = static_cast<unsigned>(g->sm_count) * 8;
             if (r->hist_width == 2) hist_pack_kernel<uint16_t><<<grid, 256, 0, st>>>(io.q_hist, nq, hc, g->d_hist_packed.as<uint16_t>());
             else hist_pack_kernel<uint32_t><<<grid, 256, 0, st>>>(io.q_hist, nq, hc, g->d_hist_packed.as<uint32_t>());
@@ -1113,8 +1115,8 @@ static int walk_collect(abb_graph *g, const abb_walk_spec *spec, const abb_walk_
     if (fl & ABB_WALK_PARENTS) acc(d2h(r->parent, io.parent, tn * 4));
     if (fl & ABB_WALK_DEPTHS) acc(d2h(r->depth, io.depth, tn * 4));
     if (e == cudaSuccess && sync) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) { abb_walk_result_free(r); return fail(ABB_ERR_CUDA, "D2H failed: %s", cudaGetErrorString(e)); }
-    *out = r;
+    if (e != cudaSuccess) return fail(ABB_ERR_CUDA, "D2H failed: %s", cudaGetErrorString(e));
+    *out = r.release();
     return ABB_OK;
 }
 
@@ -1157,7 +1159,7 @@ static int walk_host_chunked(abb_graph *g, const abb_walk_spec *spec, const int3
     const bool have_hint = g->chunk_hint_nq == nq && static_cast<int>(g->chunk_hint.size()) == K;
     // host arena: last total plus slack (the one-piece zero-copy pass pads slices, so its total is an upper bound already)
     const int64_t host_cap = g->plain_nodes + g->plain_nodes / (have_hint ? 64 : 8) + 4096ll * K;
-    std::unique_ptr<abb_walk_result, void (*)(abb_walk_result *)> r(new abb_walk_result(), abb_walk_result_free);
+    std::unique_ptr<abb_walk_result> r(new abb_walk_result());
     r->nq = nq; r->flags = fl;
     if (!(r->q_start.alloc(q * 8) && r->q_count.alloc(q * 4) && r->q_maxd.alloc(q * 4) && r->q_flags.alloc(q * 4) && r->nodes.alloc(static_cast<size_t>(host_cap) * 4)))
         return fail(ABB_ERR_NOMEM, "pinned host allocation failed");
@@ -1317,10 +1319,8 @@ extern "C" int abb_walk_host(abb_graph *g, const abb_walk_spec *spec, const int3
     g->last_host_chunks = 1;
     abb_walk_io io{}; unsigned long long totals[3] = {0, 0, 0}; int64_t h2d = 0;
     HostBlock direct;
-    if (int rc = walk_device_stage(g, spec, roots, root_off, targets, n_queries, &io, totals, &h2d, &direct)) { direct.release(); return rc; }
-    int rc = walk_collect(g, spec, io, totals, h2d, out, true, &direct);
-    direct.release();
-    return rc;
+    if (int rc = walk_device_stage(g, spec, roots, root_off, targets, n_queries, &io, totals, &h2d, &direct)) return rc;
+    return walk_collect(g, spec, io, totals, h2d, out, true, &direct);
 }
 
 // ------------------------------------------------------------------ exposure-path rows
@@ -1490,13 +1490,7 @@ struct abb_paths_result {
     bool expanded = false;
     HostBlock hops, rels, ncred, ntool;
 };
-extern "C" void abb_paths_result_free(abb_paths_result *r) {
-    if (!r) return;
-    for (HostBlock *b : {&r->off, &r->link_off, &r->link_vs, &r->link_rel, &r->link_roff, &r->link_toff, &r->t_row, &r->t_rel, &r->findings, &r->hops, &r->rels,
-                         &r->ncred, &r->ntool})
-        b->release();
-    delete r;
-}
+extern "C" void abb_paths_result_free(abb_paths_result *r) { delete r; }
 
 // links x templates -> flat rows (same layout the device's replicate kernel writes), threads over link ranges
 static bool paths_expand(abb_paths_result *r) {
@@ -1559,20 +1553,20 @@ extern "C" int64_t abb_paths_result_d2h_bytes(const abb_paths_result *r) { retur
 // findings already on the device (d_findings) or staged from the host
 static int paths_run(abb_graph *g, const int32_t *h_findings, const int32_t *d_findings, int64_t nf, abb_paths_result **out, cudaStream_t st = nullptr) {
     if (!st) st = g->stream;
-    abb_paths_result *r = new abb_paths_result();
+    std::unique_ptr<abb_paths_result> r(new abb_paths_result());
     r->nf = nf;
-    if (!r->findings.alloc(static_cast<size_t>(nf + 1) * 4)) { abb_paths_result_free(r); return fail(ABB_ERR_NOMEM, "pinned host allocation failed"); }
+    if (!r->findings.alloc(static_cast<size_t>(nf + 1) * 4)) return fail(ABB_ERR_NOMEM, "pinned host allocation failed");
     if (nf) memcpy(r->findings.p, h_findings, static_cast<size_t>(nf) * 4);
     if (!d_findings) {
-        if (int rc = g->p_findings.ensure(static_cast<size_t>(nf + 1) * 4)) { abb_paths_result_free(r); return rc; }
+        if (int rc = g->p_findings.ensure(static_cast<size_t>(nf + 1) * 4)) return rc;
         if (nf) { CUDA_TRY(cudaMemcpyAsync(g->p_findings.p, h_findings, static_cast<size_t>(nf) * 4, cudaMemcpyHostToDevice, st)); r->h2d += nf * 4; }
         d_findings = g->p_findings.as<int32_t>();
     }
-    if (int rc = g->p_off.ensure(static_cast<size_t>(nf + 1) * 8)) { abb_paths_result_free(r); return rc; }
+    if (int rc = g->p_off.ensure(static_cast<size_t>(nf + 1) * 8)) return rc;
     abb_paths_io io{};
     io.n_findings = nf; io.findings = d_findings; io.f_off = g->p_off.as<int64_t>();
     CUDA_TRY(cudaEventRecord(g->ev[2], st));
-    if (int rc = enqueue_paths_count(g, &io, st)) { abb_paths_result_free(r); return rc; }
+    if (int rc = enqueue_paths_count(g, &io, st)) return rc;
     CUDA_TRY(cudaEventRecord(g->ev[3], st));
     g->paths_timed = true;
     const PathsArgs &A = g->paths_args;
@@ -1580,7 +1574,7 @@ static int paths_run(abb_graph *g, const int32_t *h_findings, const int32_t *d_f
     r->n_links = g->paths_n_links; r->n_trows = g->paths_n_template_rows;
     bool ok = r->off.alloc(n1 * 8) && r->link_off.alloc(n1 * 8) && r->link_vs.alloc(NL * 4) && r->link_rel.alloc(NL) && r->link_roff.alloc((NL + 1) * 8) &&
               r->link_toff.alloc(NL * 8) && r->t_row.alloc(TR * 16) && r->t_rel.alloc(TR * 2);
-    if (!ok) { abb_paths_result_free(r); return fail(ABB_ERR_NOMEM, "pinned host allocation failed"); }
+    if (!ok) return fail(ABB_ERR_NOMEM, "pinned host allocation failed");
     cudaError_t e = cudaSuccess;
     auto d2h = [&](HostBlock &dst, const void *src, size_t bytes) {
         if (e == cudaSuccess && bytes) e = cudaMemcpyAsync(dst.p, src, bytes, cudaMemcpyDeviceToHost, st);
@@ -1589,9 +1583,9 @@ static int paths_run(abb_graph *g, const int32_t *h_findings, const int32_t *d_f
     d2h(r->off, io.f_off, n1 * 8); d2h(r->link_off, A.link_off, n1 * 8); d2h(r->link_vs, A.link_vs, NL * 4); d2h(r->link_rel, A.link_rel, NL);
     d2h(r->link_roff, A.link_roff, (NL + 1) * 8); d2h(r->link_toff, A.link_toff, NL * 8); d2h(r->t_row, A.t_row, TR * 16); d2h(r->t_rel, A.t_rel, TR * 2);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) { abb_paths_result_free(r); return fail(ABB_ERR_CUDA, "paths D2H failed: %s", cudaGetErrorString(e)); }
+    if (e != cudaSuccess) return fail(ABB_ERR_CUDA, "paths D2H failed: %s", cudaGetErrorString(e));
     r->rows = r->off.as<int64_t>()[nf];
-    *out = r;
+    *out = r.release();
     return ABB_OK;
 }
 
@@ -1622,16 +1616,6 @@ extern "C" const int32_t *abb_rank_result_ntool(const abb_rank_result *r) { retu
 extern "C" const uint32_t *abb_rank_result_risk_rank(const abb_rank_result *r) { return r->risk_rank.data(); }
 extern "C" const int64_t *abb_rank_result_row(const abb_rank_result *r) { return r->row.data(); }
 
-struct ScopedDev {   // scoped device allocation for the ranking pass (sizes follow the row count)
-    void *p = nullptr;
-    ~ScopedDev() { if (p) cudaFree(p); }
-    int alloc(size_t bytes) {
-        cudaError_t e = cudaMalloc(&p, bytes ? bytes : 16);
-        return e == cudaSuccess ? ABB_OK : fail(ABB_ERR_NOMEM, "cudaMalloc(%zu): %s", bytes, cudaGetErrorString(e));
-    }
-    template <class T> T *as() const { return static_cast<T *>(p); }
-};
-
 // One ranking path: node_focus == nullptr ranks every row (abb_paths_rank_host); otherwise the rows that miss the focus are
 // compacted away (cub::DeviceSelect keeps their order) and only the matched rows are sorted.
 static int paths_rank(abb_graph *g, const int32_t *findings, int64_t n_findings, const int32_t *base_id, const uint32_t *risk_rank, int64_t n_base,
@@ -1647,7 +1631,7 @@ static int paths_rank(abb_graph *g, const int32_t *findings, int64_t n_findings,
     const bool focused = node_focus != nullptr;
     if (int rc = g->p_findings.ensure(static_cast<size_t>(nf + 1) * 4)) return rc;
     if (int rc = g->p_off.ensure(static_cast<size_t>(nf + 1) * 8)) return rc;
-    ScopedDev d_base, d_tab, d_ncu, d_ntu, d_focus;
+    DevBuf d_base, d_tab, d_ncu, d_ntu, d_focus;
     if (int rc = d_base.alloc(static_cast<size_t>(nf + 1) * 4)) return rc;
     if (int rc = d_tab.alloc(static_cast<size_t>(n_base) * 75 * 4)) return rc;
     if (int rc = d_ncu.alloc(static_cast<size_t>(n + 1) * 4)) return rc;
@@ -1668,17 +1652,17 @@ static int paths_rank(abb_graph *g, const int32_t *findings, int64_t n_findings,
     CUDA_TRY(cudaMemcpyAsync(&R, io.f_off + nf, 8, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     if (R >= (1ll << 32) - 1) return fail(ABB_ERR_CAPACITY, "more than 2^32 exposure-path rows in one ranking batch");
-    abb_rank_result *r = new abb_rank_result();
+    std::unique_ptr<abb_rank_result> r(new abb_rank_result());
     r->total = R;
     r->matched = R;
     // unfocused, the page is known before any kernel runs; focused, the matched count is needed first
-    if (R == 0 || (!focused && std::min(limit, R - std::min(offset, R)) == 0)) { r->matched = focused ? 0 : R; *out = r; return ABB_OK; }
-    ScopedDev k1, k2, v1, v2, tmp, d_sel, sel_tmp;
+    if (R == 0 || (!focused && std::min(limit, R - std::min(offset, R)) == 0)) { r->matched = focused ? 0 : R; *out = r.release(); return ABB_OK; }
+    DevBuf k1, k2, v1, v2, tmp, d_sel, sel_tmp;
     int rc = k1.alloc(static_cast<size_t>(R) * 8);
     if (!rc) rc = k2.alloc(static_cast<size_t>(R) * 8);
     if (!rc) rc = v1.alloc(static_cast<size_t>(R) * 4);
     if (!rc) rc = v2.alloc(static_cast<size_t>(R) * 4);
-    if (rc) { delete r; return rc; }
+    if (rc) return rc;
     PathsArgs A = g->paths_args;
     RankArgs RA{d_base.as<int32_t>(), d_tab.as<uint32_t>(), d_ncu.as<int32_t>(), d_ntu.as<int32_t>(), k1.as<unsigned long long>(), v1.as<uint32_t>(),
                 d_focus.as<uint8_t>(), io.findings, need};
@@ -1698,9 +1682,9 @@ static int paths_rank(abb_graph *g, const int32_t *findings, int64_t n_findings,
         int64_t M = 0;
         if (!rc && ce == cudaSuccess) ce = cudaMemcpyAsync(&M, d_sel.p, 8, cudaMemcpyDeviceToHost, st);
         if (!rc && ce == cudaSuccess) ce = cudaStreamSynchronize(st);
-        if (rc || ce != cudaSuccess) { delete r; return rc ? rc : fail(ABB_ERR_CUDA, "focus compaction failed: %s", cudaGetErrorString(ce)); }
+        if (rc || ce != cudaSuccess) return rc ? rc : fail(ABB_ERR_CUDA, "focus compaction failed: %s", cudaGetErrorString(ce));
         r->matched = M;
-        if (M == 0 || std::min(limit, M - std::min(offset, M)) == 0) { *out = r; return ABB_OK; }
+        if (M == 0 || std::min(limit, M - std::min(offset, M)) == 0) { *out = r.release(); return ABB_OK; }
         gather_keys_kernel<<<static_cast<unsigned>((M + 255) / 256), 256, 0, st>>>(k1.as<unsigned long long>(), v2.as<uint32_t>(), M, k2.as<unsigned long long>());
         g_launches++;
         std::swap(key_in, key_out); std::swap(row_in, row_out);
@@ -1713,15 +1697,15 @@ static int paths_rank(abb_graph *g, const int32_t *findings, int64_t n_findings,
     if (ce == cudaSuccess && !(rc = tmp.alloc(tb)))
         ce = cub::DeviceRadixSort::SortPairs(tmp.p, tb, key_in, key_out, row_in, row_out, static_cast<int>(M), 0, 64, st);
     g_launches++;
-    if (rc || ce != cudaSuccess) { delete r; return rc ? rc : fail(ABB_ERR_CUDA, "radix sort failed: %s", cudaGetErrorString(ce)); }
-    ScopedDev o_hops, o_rels, o_nc, o_nt, o_rank, o_row;
+    if (rc || ce != cudaSuccess) return rc ? rc : fail(ABB_ERR_CUDA, "radix sort failed: %s", cudaGetErrorString(ce));
+    DevBuf o_hops, o_rels, o_nc, o_nt, o_rank, o_row;
     rc = o_hops.alloc(static_cast<size_t>(count) * 16);
     if (!rc) rc = o_rels.alloc(static_cast<size_t>(count) * 4);
     if (!rc) rc = o_nc.alloc(static_cast<size_t>(count) * 4);
     if (!rc) rc = o_nt.alloc(static_cast<size_t>(count) * 4);
     if (!rc) rc = o_rank.alloc(static_cast<size_t>(count) * 4);
     if (!rc) rc = o_row.alloc(static_cast<size_t>(count) * 8);
-    if (rc) { delete r; return rc; }
+    if (rc) return rc;
     A.io.hops = o_hops.as<int32_t>(); A.io.rels = o_rels.as<int8_t>(); A.io.ncred = o_nc.as<int32_t>(); A.io.ntool = o_nt.as<int32_t>(); A.io.row_cap = count;
     rank_gather_kernel<<<static_cast<unsigned>((count + 255) / 256), 256, 0, st>>>(A, RA, row_out, first, count, o_rank.as<uint32_t>(), o_row.as<int64_t>());
     g_launches++;
@@ -1735,8 +1719,8 @@ static int paths_rank(abb_graph *g, const int32_t *findings, int64_t n_findings,
     if (ce == cudaSuccess) ce = cudaMemcpyAsync(r->risk_rank.data(), o_rank.p, static_cast<size_t>(count) * 4, cudaMemcpyDeviceToHost, st);
     if (ce == cudaSuccess) ce = cudaMemcpyAsync(r->row.data(), o_row.p, static_cast<size_t>(count) * 8, cudaMemcpyDeviceToHost, st);
     if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
-    if (ce != cudaSuccess) { delete r; return fail(ABB_ERR_CUDA, "ranking failed: %s", cudaGetErrorString(ce)); }
-    *out = r;
+    if (ce != cudaSuccess) return fail(ABB_ERR_CUDA, "ranking failed: %s", cudaGetErrorString(ce));
+    *out = r.release();
     return ABB_OK;
 }
 
@@ -1786,13 +1770,12 @@ extern "C" int abb_exposure_host(abb_graph *g, const int32_t *findings, int64_t 
         t1 = now();
         if (!rc) rc = walk_collect(g, &spec, io, totals, h2d, &wr, true, &direct);
     }
-    direct.release();
     const auto t2 = now();
     helper.join();
     const auto t3 = now();
     if (rc || prc) {
-        if (wr) abb_walk_result_free(wr);
-        if (pr) abb_paths_result_free(pr);
+        delete wr;
+        delete pr;
         if (!rc) { g_err = perr; return prc; }
         return rc;
     }
@@ -1805,23 +1788,18 @@ extern "C" int abb_exposure_host(abb_graph *g, const int32_t *findings, int64_t 
 struct abb_finding_context_result {
     int64_t nq = 0, total = 0, h2d = 0, d2h = 0;
     float walk_ms = -1.f, context_ms = -1.f;
-    abb_walk_result *walk = nullptr;   // count / maxd / flags / histogram of the impact walk; no slices
+    std::unique_ptr<abb_walk_result> walk;   // count / maxd / flags / histogram of the impact walk; no slices
     HostBlock start, bcnt, src;
 };
-extern "C" void abb_finding_context_result_free(abb_finding_context_result *r) {
-    if (!r) return;
-    abb_walk_result_free(r->walk);
-    for (HostBlock *b : {&r->start, &r->bcnt, &r->src}) b->release();
-    delete r;
-}
+extern "C" void abb_finding_context_result_free(abb_finding_context_result *r) { delete r; }
 extern "C" int64_t abb_finding_context_result_queries(const abb_finding_context_result *r) { return r->nq; }
-extern "C" const int32_t *abb_finding_context_result_count(const abb_finding_context_result *r) { return abb_walk_result_count(r->walk); }
-extern "C" const int32_t *abb_finding_context_result_maxd(const abb_finding_context_result *r) { return abb_walk_result_maxd(r->walk); }
-extern "C" const int32_t *abb_finding_context_result_flags(const abb_finding_context_result *r) { return abb_walk_result_flags(r->walk); }
+extern "C" const int32_t *abb_finding_context_result_count(const abb_finding_context_result *r) { return abb_walk_result_count(r->walk.get()); }
+extern "C" const int32_t *abb_finding_context_result_maxd(const abb_finding_context_result *r) { return abb_walk_result_maxd(r->walk.get()); }
+extern "C" const int32_t *abb_finding_context_result_flags(const abb_finding_context_result *r) { return abb_walk_result_flags(r->walk.get()); }
 extern "C" const void *abb_finding_context_result_hist_packed(const abb_finding_context_result *r, uint32_t *columns_mask, int32_t *bytes_per_count) {
-    return abb_walk_result_hist_packed(r->walk, columns_mask, bytes_per_count);
+    return abb_walk_result_hist_packed(r->walk.get(), columns_mask, bytes_per_count);
 }
-extern "C" const uint32_t *abb_finding_context_result_hist(const abb_finding_context_result *r) { return abb_walk_result_hist(r->walk); }
+extern "C" const uint32_t *abb_finding_context_result_hist(const abb_finding_context_result *r) { return abb_walk_result_hist(r->walk.get()); }
 extern "C" const int64_t *abb_finding_context_result_start(const abb_finding_context_result *r) { return r->start.as<int64_t>(); }
 extern "C" const int32_t *abb_finding_context_result_bucket_counts(const abb_finding_context_result *r) { return r->bcnt.as<int32_t>(); }
 extern "C" int64_t abb_finding_context_result_total_sources(const abb_finding_context_result *r) { return r->total; }
@@ -1848,7 +1826,7 @@ extern "C" int abb_finding_context_host(abb_graph *g, int32_t max_depth, const i
 #define ENS(buf, bytes) if (!rc) rc = g->buf.ensure(static_cast<size_t>(bytes))
     ENS(d_roots, q1 * 4); ENS(cx_bcnt, q1 * CTX_BUCKETS * 4); ENS(cx_cnt, q1 * 8); ENS(cx_start, q1 * 8);
     if (rc) return rc;
-    std::unique_ptr<abb_finding_context_result, void (*)(abb_finding_context_result *)> r(new abb_finding_context_result(), abb_finding_context_result_free);
+    std::unique_ptr<abb_finding_context_result> r(new abb_finding_context_result());
     r->nq = nq;
     if (nq) CUDA_TRY(cudaMemcpyAsync(g->d_roots.p, findings, q * 4, cudaMemcpyHostToDevice, st));
     r->h2d = nq * 4;
@@ -1891,7 +1869,9 @@ extern "C" int abb_finding_context_host(abb_graph *g, int32_t max_depth, const i
     };
     d2h(r->start, g->cx_start.p, q * 8); d2h(r->bcnt, g->cx_bcnt.p, q * CTX_BUCKETS * 4); d2h(r->src, g->cx_src.p, static_cast<size_t>(total) * 4);
     if (e != cudaSuccess) { drain(); return fail(ABB_ERR_CUDA, "finding context failed: %s", cudaGetErrorString(e)); }
-    if ((rc = walk_collect(g, &spec, io, totals, wh2d, &r->walk, true, nullptr, false))) { drain(); return rc; }
+    abb_walk_result *walk = nullptr;
+    if ((rc = walk_collect(g, &spec, io, totals, wh2d, &walk, true, nullptr, false))) { drain(); return rc; }
+    r->walk.reset(walk);
     if ((e = cudaStreamSynchronize(cs)) != cudaSuccess) { drain(); return fail(ABB_ERR_CUDA, "finding context failed: %s", cudaGetErrorString(e)); }
     r->d2h += r->walk->d2h;
     float a = 0.f, b = 0.f;
