@@ -336,7 +336,9 @@ def test_empty_and_ragged_batches():
 
 
 def test_whole_graph_walks_reach_the_last_tier():
-    """Unbounded walks over a dense seeded graph outgrow the shared-memory and bounded-queue tiers (S1 -> G1 -> GX)."""
+    """Unbounded walks over a dense seeded graph outgrow the shared-memory and bounded-queue tiers (S1 -> G1 -> GX).  G1's queue
+    (n + 4096 entries here) holds any walk of this graph, so it is G1's level forecast that hands them to GX; the 70 000-node chain
+    of test_gpu_graph_shapes.py fills G1's queue instead."""
     og, dg, _, _, _ = graphs_for((30000, 400000, 4))
     rng = np.random.default_rng(29)
     sources = rng.integers(0, og.n_nodes, size=12).astype(np.int32)
@@ -345,6 +347,8 @@ def test_whole_graph_walks_reach_the_last_tier():
     for dedup in (True, False):
         dg.set_dedup(dedup)
         got = dg.walk(dg.spec_distances(0xFFFFFFFF), sources)
+        t = dg.last_walk_tier_counts()["first"]
+        assert t["s1"] == len(sources) and t["g1"] > 0, t
         assert_slices_equal(got, want, gpu_aux="depth")
     dg.set_dedup(True)
     spec = dg.spec_traverse(3, 12, -1, -1, False, 0, False, False, True)
@@ -352,5 +356,7 @@ def test_whole_graph_walks_reach_the_last_tier():
     root_off = np.arange(5, dtype=np.int64)
     want_t = orc.traverse_many(og, roots, root_off, direction=3, max_depth=12)
     got_t = dg.walk(spec, roots, root_off)
+    t = dg.last_walk_tier_counts()["first"]
+    assert t["s1"] == len(roots) and t["g1"] > 0, t
     assert_slices_equal(got_t, want_t, gpu_aux="depth")
     np.testing.assert_array_equal(got_t.ecount, np.diff(want_t.eoff))
