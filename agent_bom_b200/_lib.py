@@ -181,6 +181,14 @@ EXPORTS = {
     "abb_reach_vuln_minhop": (vp, [vp]),
     "abb_reach_result_free": (None, [vp]),
     "abb_bottleneck_host": (C.c_int, [vp, vp, i64, vp]),
+    "abb_pagerank_host": (C.c_int, [vp, vp, vp, vp]),
+    "abb_betweenness_host": (C.c_int, [vp, vp]),
+    "abb_bidir_paths_host": (C.c_int, [vp, vp, vp, i64, C.POINTER(vp)]),
+    "abb_bidir_result_start": (vp, [vp]),
+    "abb_bidir_result_length": (vp, [vp]),
+    "abb_bidir_result_total": (i64, [vp]),
+    "abb_bidir_result_nodes": (vp, [vp]),
+    "abb_bidir_result_free": (None, [vp]),
     "abb_lateral_paths_host": (C.c_int, [C.c_int, i32, vp, vp, vp, vp, vp, i64, vp, vp, i32, i64, C.POINTER(vp)]),
     "abb_lateral_result_off": (vp, [vp]),
     "abb_lateral_result_records": (vp, [vp]),

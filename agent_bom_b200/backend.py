@@ -7,6 +7,10 @@ discovery order, ``shortest_path`` the first-discoverer path, ``centrality_score
 ``bottleneck_nodes`` the 50-source sampled score.  The traversals (``bfs``, ``shortest_path``, ``bottleneck_nodes``)
 run on the GPU through the ordered walk engine; the adjacency is exported to a CSR lazily and re-exported after a
 mutation.  ``get_backend`` / ``from_context_graph`` / ``from_unified_graph`` mirror ``:245-306``.
+
+B200NetworkXBackend (name ``"b200-networkx"``) is the drop-in for the reference's other backend, ``NetworkXBackend``
+(``:158-242``): an ``nx.DiGraph`` on the host, with PageRank, exact betweenness and NetworkX's bidirectional shortest paths
+computed on the GPU.
 """
 
 from __future__ import annotations
@@ -187,6 +191,162 @@ class B200Backend:
         return from_unified_graph(graph, device=device)
 
 
+class B200NetworkXBackend:
+    """Drop-in for ``NetworkXBackend`` (graph_backend.py:158-242) with the host semantics of an ``nx.DiGraph``: ``add_edge``
+    creates missing endpoints as attribute-less nodes; adding a node or an edge again merges its attributes into the existing
+    entry, which keeps its position; ``edge_count`` is ``number_of_edges() // 2`` (the reference's count, also for directed-only
+    graphs).  ``centrality_scores`` is ``nx.pagerank``, ``bottleneck_nodes`` exact ``nx.betweenness_centrality``, ``bfs`` /
+    ``shortest_path`` use ``nx.shortest_path``'s bidirectional search — all on the GPU, bit for bit with networkx 3.6.1."""
+
+    name = "b200-networkx"
+
+    def __init__(self, device: int = 0):
+        self._nodes: dict[str, dict] = {}
+        self._succ: dict[str, dict[str, dict]] = {}
+        self._edges: list[tuple[str, str]] = []     # first insertion order: rows of both CSR directions keep dict order
+        self._device = device
+        self._csr: csrmod.HostCSR | None = None
+        self._weights: np.ndarray | None = None
+        self._dg = None
+
+    # ── mutation ────────────────────────────────────────────────────────
+    def _invalidate(self) -> None:
+        self._csr = self._weights = None
+        if self._dg is not None:
+            self._dg.close()
+            self._dg = None
+
+    def _ensure_node(self, node_id: str) -> dict:
+        data = self._nodes.get(node_id)
+        if data is None:
+            data = self._nodes[node_id] = {}
+            self._succ[node_id] = {}
+            self._invalidate()
+        return data
+
+    def _put_edge(self, source: str, target: str, attrs: dict) -> None:
+        self._ensure_node(source)
+        self._ensure_node(target)
+        row = self._succ[source]
+        if target not in row:
+            row[target] = {}
+            self._edges.append((source, target))
+        row[target].update(attrs)
+
+    def add_node(self, node_id: str, kind: str, label: str, **metadata: object) -> None:
+        self._ensure_node(node_id).update({"kind": kind, "label": label, **metadata})
+
+    def add_edge(self, source: str, target: str, kind: str, weight: float = 1.0, *, directed: bool = False, **metadata: object) -> None:
+        self._put_edge(source, target, {"kind": kind, "weight": weight, **metadata})
+        if not directed:
+            self._put_edge(target, source, {"kind": kind, "weight": weight, **metadata})
+        self._invalidate()                  # a merged weight changes PageRank even when the topology does not
+
+    # ── point queries (host) ────────────────────────────────────────────
+    def has_node(self, node_id: str) -> bool:
+        return node_id in self._nodes
+
+    def has_edge(self, source: str, target: str) -> bool:
+        return target in self._succ.get(source, {})
+
+    def neighbors(self, node_id: str) -> list[str]:
+        return list(self._succ.get(node_id, {}))
+
+    def node_count(self) -> int:
+        return len(self._nodes)
+
+    def edge_count(self) -> int:
+        return len(self._edges) // 2
+
+    def to_dict(self) -> dict:
+        seen: set[tuple[str, str]] = set()
+        edges = []
+        for src, targets in self._succ.items():
+            for tgt, data in targets.items():
+                key = (min(src, tgt), max(src, tgt))
+                if key not in seen:
+                    seen.add(key)
+                    edges.append({"source": src, "target": tgt, **data})
+        return {
+            "nodes": [{"id": nid, **data} for nid, data in self._nodes.items()],
+            "edges": edges,
+            "stats": {"node_count": self.node_count(), "edge_count": self.edge_count()},
+        }
+
+    # ── device export ───────────────────────────────────────────────────
+    @property
+    def csr(self) -> csrmod.HostCSR:
+        """The DiGraph in node order: forward rows = successors, reverse rows = predecessors, both in dict order."""
+        if self._csr is None:
+            ids = list(self._nodes)
+            index = {nid: i for i, nid in enumerate(ids)}
+            ne = len(self._edges)
+            src = np.fromiter((index[s] for s, _ in self._edges), dtype=np.int32, count=ne)
+            dst = np.fromiter((index[t] for _, t in self._edges), dtype=np.int32, count=ne)
+            c = csrmod.from_arrays(ids, np.zeros(len(ids), dtype=np.uint8), src, dst, np.zeros(ne, dtype=np.uint8),
+                                   np.full(ne, csrmod.EDGE_TRAVERSABLE, dtype=np.uint8))
+            c.index = index
+            self._csr = c
+        return self._csr
+
+    @property
+    def weights(self) -> np.ndarray:
+        """``weight`` of each forward adjacency entry as f64 (NetworkX reads ``d.get("weight", 1)``)."""
+        if self._weights is None:
+            c = self.csr
+            by_edge = np.fromiter((float(self._succ[s][t].get("weight", 1)) for s, t in self._edges), dtype=np.float64, count=len(self._edges))
+            self._weights = np.ascontiguousarray(by_edge[c.fwd_eid >> 1])
+        return self._weights
+
+    @property
+    def device_graph(self):
+        if self._dg is None:
+            from .engine import DeviceGraph
+
+            self._dg = DeviceGraph.upload(self.csr, self._device)
+        return self._dg
+
+    # ── analytics (GPU) ─────────────────────────────────────────────────
+    def bfs(self, source: str, max_depth: int = 4) -> list[list[str]]:
+        """``nx.shortest_path(G, source, v)`` for every node ``v`` of ``nx.bfs_tree(G, source, depth_limit=max_depth)`` but the
+        source, in the tree's discovery order: one ordered walk for the tree, one batched bidirectional search for the paths."""
+        if source not in self._nodes:
+            return []
+        c = self.csr
+        s = c.index[source]
+        tree = self.device_graph.bfs_many(np.asarray([s], dtype=np.int32), max_depth, False).slice(0)
+        paths = self.device_graph.bidirectional_paths(np.full(tree.shape[0], s, dtype=np.int32), tree)
+        ids = c.node_ids
+        return [[ids[int(u)] for u in p] for p in paths]
+
+    def shortest_path(self, source: str, target: str) -> list[str] | None:
+        if source not in self._nodes or target not in self._nodes:
+            return None
+        if source == target:
+            return [source]
+        c = self.csr
+        p = self.device_graph.bidirectional_paths(np.asarray([c.index[source]], dtype=np.int32), np.asarray([c.index[target]], dtype=np.int32))[0]
+        return None if p is None else [c.node_ids[int(u)] for u in p]
+
+    def centrality_scores(self) -> dict[str, float]:
+        """``nx.pagerank(G)``: alpha 0.85, 100 iterations at most, tolerance 1e-6, edge weights."""
+        if not self._nodes:
+            return {}
+        scores, _ = self.device_graph.pagerank(self.weights)
+        return dict(zip(self.csr.node_ids, scores.tolist()))
+
+    def bottleneck_nodes(self, top_n: int = 5) -> list[tuple[str, float]]:
+        """Exact ``nx.betweenness_centrality(G)``, highest first, ties in node order."""
+        if not self._nodes:
+            return []
+        scores = self.device_graph.betweenness()
+        return sorted(zip(self.csr.node_ids, scores.tolist()), key=lambda x: x[1], reverse=True)[:top_n]
+
+    @classmethod
+    def from_unified_graph(cls, graph, device: int = 0) -> "B200NetworkXBackend":
+        return from_unified_graph(graph, backend=cls.name, device=device)
+
+
 def rank_bottlenecks(c: csrmod.HostCSR, scores: np.ndarray, top_n: int) -> list[tuple[str, float]]:
     """Normalise and rank raw device scores the way the reference does; a scored id without a node record is the
     reference's ``KeyError`` (its score table only holds recorded nodes)."""
@@ -199,15 +359,18 @@ def rank_bottlenecks(c: csrmod.HostCSR, scores: np.ndarray, top_n: int) -> list[
     return [(c.node_ids[int(i)], float(real[int(i)]) / total) for i in order]
 
 
-def get_backend(backend: str = "b200", **kwargs) -> B200Backend:
+def get_backend(backend: str = "b200", **kwargs) -> B200Backend | B200NetworkXBackend:
     """``get_backend("b200")`` — the name a ``--graph-backend b200`` flag would pass (reference cli/options_surfaces.py:161-162;
-    factory ``graph_backend.py:245-259``).  There is no CPU fallback here: other names are an error."""
+    factory ``graph_backend.py:245-259``); ``"b200-networkx"`` gives the NetworkXBackend drop-in.  There is no CPU fallback
+    here: other names are an error."""
     if backend in ("b200", "auto"):
         return B200Backend(**kwargs)
-    raise ValueError(f"unknown graph backend {backend!r}: this package only provides 'b200' (no CPU fallback)")
+    if backend == B200NetworkXBackend.name:
+        return B200NetworkXBackend(**kwargs)
+    raise ValueError(f"unknown graph backend {backend!r}: this package only provides 'b200' and 'b200-networkx' (no CPU fallback)")
 
 
-def from_context_graph(context_graph_data: dict, backend: str = "b200", **kwargs) -> B200Backend:
+def from_context_graph(context_graph_data: dict, backend: str = "b200", **kwargs) -> B200Backend | B200NetworkXBackend:
     """Serialised context graph → backend (``:262-278``): undirected edges, kind / label / weight kept."""
     graph = get_backend(backend, **kwargs)
     for node in context_graph_data.get("nodes", []):
@@ -217,7 +380,7 @@ def from_context_graph(context_graph_data: dict, backend: str = "b200", **kwargs
     return graph
 
 
-def from_unified_graph(ug, backend: str = "b200", **kwargs) -> B200Backend:
+def from_unified_graph(ug, backend: str = "b200", **kwargs) -> B200Backend | B200NetworkXBackend:
     """UnifiedGraph → backend (``:281-306``): directed edges one-way, bidirectional edges both ways."""
     graph = get_backend(backend, **kwargs)
     for node in ug.nodes.values():

@@ -28,6 +28,7 @@
 #include "reach.cuh"
 #include "union.cuh"
 #include "centrality.cuh"
+#include "nxcentral.cuh"
 #include "lateral.cuh"
 #include "walk.cuh"
 #include "walkb.cuh"
@@ -222,6 +223,7 @@ struct abb_graph {
     int big_grid = 0;
     int mid_warps = 8;                // ABB_MID_WARPS=4: 4-warp mid blocks
     int64_t big_limit = 0;            // the big tier takes S1's heavy hand-offs when there are at most this many (default 24 per SM)
+    int64_t nx_batch = 0;             // cap on betweenness sources per batch and on path-search slots (0: sized from free memory)
     DevBuf b_gq, b_gpar, b_gdep;
     // tier G1: many per-warp slots (bitmap over all nodes + a bounded queue); tier GX: a few slots that can hold a whole-graph walk
     DevBuf g_bitmap, g_queue, g_par, g_dep;
@@ -460,6 +462,9 @@ extern "C" int abb_graph_set_option(abb_graph *g, const char *name, int64_t valu
     else if (k == "big_limit") {
         if (value < 0) return fail(ABB_ERR_ARG, "big_limit must be >= 0");
         g->big_limit = value;
+    } else if (k == "nx_batch") {
+        if (value < 0) return fail(ABB_ERR_ARG, "nx_batch must be >= 0");
+        g->nx_batch = value;
     } else return fail(ABB_ERR_ARG, "unknown option '%s'", name);
     return ABB_OK;
 }
@@ -476,6 +481,7 @@ extern "C" int64_t abb_graph_get_option(const abb_graph *g, const char *name) {
     if (k == "chunk_min") return g->chunk_min;
     if (k == "last_host_chunks") return g->last_host_chunks;
     if (k == "big_limit") return g->big_limit;
+    if (k == "nx_batch") return g->nx_batch;
     return -1;
 }
 
@@ -1884,4 +1890,5 @@ extern "C" int abb_finding_context_host(abb_graph *g, int32_t max_depth, const i
 #include "reach_host.inl"
 #include "union_host.inl"
 #include "centrality_host.inl"
+#include "nxcentral_host.inl"
 #include "lateral_host.inl"

@@ -533,6 +533,44 @@ class DeviceGraph:
             _lib.check(_lib.load().abb_bottleneck_host(h, src.ctypes.data, int(src.shape[0]), out.ctypes.data))
         return out
 
+    # ── NetworkX analysis backend ───────────────────────────────────────
+    def pagerank(self, weights) -> tuple[np.ndarray, int]:
+        """``nx.pagerank`` of the graph as a DiGraph (``abb_pagerank_host``): f64 score per node and the power iterations run.
+        ``weights``: f64 edge weight per forward adjacency entry."""
+        w = np.ascontiguousarray(weights, dtype=np.float64)
+        if w.shape[0] != self.n_entries:
+            raise ValueError("pagerank needs one weight per adjacency entry")
+        out = np.zeros(self.n_nodes, dtype=np.float64)
+        iters = C.c_int32(0)
+        with self._use() as h:
+            _lib.check(_lib.load().abb_pagerank_host(h, w.ctypes.data, out.ctypes.data, C.byref(iters)))
+        return out, int(iters.value)
+
+    def betweenness(self) -> np.ndarray:
+        """``nx.betweenness_centrality`` of the graph as a DiGraph (``abb_betweenness_host``): f64 per node."""
+        out = np.zeros(self.n_nodes, dtype=np.float64)
+        with self._use() as h:
+            _lib.check(_lib.load().abb_betweenness_host(h, out.ctypes.data))
+        return out
+
+    def bidirectional_paths(self, sources, targets) -> list[np.ndarray | None]:
+        """``nx.shortest_path(G, s, t)`` per pair (``abb_bidir_paths_host``): node indices source first, ``None`` when there is no path."""
+        lib = _lib.load()
+        s, t = _i32(sources), _i32(targets)
+        if s.shape != t.shape:
+            raise ValueError("sources and targets differ in length")
+        res = _vp()
+        with self._use() as h:
+            _lib.check(lib.abb_bidir_paths_host(h, s.ctypes.data, t.ctypes.data, int(s.shape[0]), C.byref(res)))
+        try:
+            n = int(s.shape[0])
+            start = _view(lib.abb_bidir_result_start(res), n, np.int64)
+            length = _view(lib.abb_bidir_result_length(res), n, np.int32)
+            nodes = _view(lib.abb_bidir_result_nodes(res), int(lib.abb_bidir_result_total(res)), np.int32)
+        finally:
+            lib.abb_bidir_result_free(res)
+        return [nodes[a: a + k] if k else None for a, k in zip(start.tolist(), length.tolist())]
+
     # ── timing hooks used by bench.py ───────────────────────────────────
     def last_walk_ms(self) -> float:
         return float(_lib.load().abb_last_walk_ms(self.handle))

@@ -422,6 +422,28 @@ void abb_reach_result_free(abb_reach_result *r);
  * sum and sorts, as the reference does).  Sources must be nodes with a record (ghost / invalid sources add nothing). */
 int abb_bottleneck_host(abb_graph *g, const int32_t *sources, int64_t n_sources, uint64_t *scores_out);
 
+/* ---- NetworkX analysis backend ----------------------------------------------------------------------------------
+ * The answers of the reference's NetworkXBackend (agent_bom/graph_backend.py:158-242), bit for bit with networkx 3.6.1.
+ * The graph is an nx.DiGraph exported in node order: forward row u = G.succ[u] in dict order, reverse row u = G.pred[u]
+ * in dict order, no row repeating a neighbour, every node real.  Option "nx_batch" caps the betweenness sources per batch and
+ * the path-search slots (results never depend on it).
+ *
+ * PageRank — nx.pagerank(G) (_pagerank_scipy, alpha 0.85, max_iter 100, tol 1e-6, weight "weight"): weights[n_entries] is
+ * the edge weight of each forward entry as f64.  scores_out: host [n_nodes]; *iterations_out: power iterations run.
+ * ABB_ERR_ARG when the iteration does not converge (networkx raises PowerIterationFailedConvergence). */
+int abb_pagerank_host(abb_graph *g, const double *weights, double *scores_out, int32_t *iterations_out);
+/* Betweenness — nx.betweenness_centrality(G): exact Brandes from every source, normalised, endpoints excluded. */
+int abb_betweenness_host(abb_graph *g, double *scores_out);
+/* Shortest paths — nx.shortest_path(G, s, t) (_bidirectional_pred_succ) for a batch of pairs of valid node indices: the path
+ * of pair q is nodes[start[q] .. start[q]+length[q]), source first; length 0 = no path; s == t gives [s]. */
+typedef struct abb_bidir_result abb_bidir_result;
+int abb_bidir_paths_host(abb_graph *g, const int32_t *sources, const int32_t *targets, int64_t n_pairs, abb_bidir_result **out);
+const int64_t *abb_bidir_result_start(const abb_bidir_result *r);   /* [n_pairs] */
+const int32_t *abb_bidir_result_length(const abb_bidir_result *r);  /* [n_pairs] */
+int64_t abb_bidir_result_total(const abb_bidir_result *r);
+const int32_t *abb_bidir_result_nodes(const abb_bidir_result *r);   /* [total] */
+void abb_bidir_result_free(abb_bidir_result *r);
+
 /* ---- lateral-movement path search -------------------------------------------------------------------------------
  * Replaces the queue loop of find_lateral_paths (agent_bom/context_graph.py:397-477) for a batch of sources: a FIFO of
  * simple paths over graph.adjacency, at most 100 recorded paths and 10 000 waiting paths per source, paths no longer
