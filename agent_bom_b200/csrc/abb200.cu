@@ -265,13 +265,16 @@ struct abb_graph {
     // graph-constant server tables (built on first use): fan-out, and the principal rows each server contributes to a template
     DevBuf srv_cred, srv_tool, srv_roff, srv_row, srv_rel;
     bool srv_table_ready = false;
+    // graph-constant exposure tables (built on first use, ensure_exposure_tables): links of every finding node, templates of every
+    // vulnerable source, rows per finding node
+    DevBuf x_vs, x_loff, x_link, x_rows, x_toff, x_trow, x_trel, x_overflow;
+    bool x_tables_ready = false;
     // paths staging
     DevBuf p_findings, p_off, p_scan_tmp;
-    // exposure-path pipeline workspace (links, templates)
-    DevBuf pl_cnt, pl_off, pl_vs, pl_rel, pl_f, pl_rows, pl_roff, pl_toff, pl_need, pl_ulist, pl_nu, pt_cnt, pt_off, pt_off_node, pt_cnt_node, pt_row, pt_rel;
+    // exposure-path per-call workspace: rows and links per finding; the host result's batch links and templates
+    DevBuf pl_cnt, pl_link, pl_lcnt, pl_off, pl_vs, pl_rel, pl_roff, pl_toff, pl_need, pl_ulist, pl_nu, pt_cnt, pt_off, pt_off_node, pt_row, pt_rel;
     PathsArgs paths_args{};
     bool paths_args_valid = false;
-    int64_t paths_n_links = 0, paths_n_template_rows = 0;
     int replicate_grid = 0, rank_keys_grid = 0;   // grids of the row-parallel kernels (row_grid)
     int64_t hint_rows = 0;
     // finding-context workspace (context.cuh): per-finding bucket counts, totals, start offsets, source lists; the context kernels run on
@@ -1385,68 +1388,85 @@ static unsigned row_grid(const abb_graph *g, K kernel, int &cached) {
     return static_cast<unsigned>(cached);
 }
 
-// Count pass of the exposure-path pipeline (paths.cuh): links -> unique vulnerable sources -> templates -> per-finding
-// row offsets.  Synchronises the stream twice to size the link / template buffers.
-static int enqueue_paths_count(abb_graph *g, const abb_paths_io *io, cudaStream_t st) {
-    NvtxRange nvtx_("paths: links / templates / offsets");
+// the graph's parts of the exposure-path arguments: server table and exposure tables
+static PathsArgs paths_base(abb_graph *g) {
+    PathsArgs A{};
+    A.g = g->v; A.srv_cred = g->srv_cred.as<int32_t>(); A.srv_tool = g->srv_tool.as<int32_t>();
+    A.srv_roff = g->srv_roff.as<int64_t>(); A.srv_row = g->srv_row.as<int4>(); A.srv_rel = g->srv_rel.as<int8_t>();
+    A.x_vs = g->x_vs.as<uint8_t>(); A.x_loff = g->x_loff.as<int64_t>(); A.x_link = g->x_link.as<LinkRec>(); A.x_rows = g->x_rows.as<int32_t>();
+    A.x_toff = g->x_toff.as<int64_t>(); A.t_row = g->x_trow.as<int4>(); A.t_rel = g->x_trel.as<int8_t>(); A.x_overflow = g->x_overflow.as<unsigned>();
+    return A;
+}
+
+// Graph-constant exposure tables (paths.cuh): the links of every finding node, the template of every vulnerable source and the
+// rows of every finding node, built once per graph (count -> scan in place -> fill) and freed with it.  Synchronises the stream
+// to size the link and template arrays, and once more at the end: later calls may come on other streams.
+static int ensure_exposure_tables(abb_graph *g, cudaStream_t st) {
+    if (g->x_tables_ready) return ABB_OK;
+    NvtxRange nvtx_("paths: graph-constant exposure tables");
+    if (int rc = ensure_server_table(g, st)) return rc;
+    const int64_t n = g->v.n;
+    const size_t n1 = static_cast<size_t>(n) + 1;
+    int rc = ABB_OK;
+    if (!rc) rc = g->x_vs.alloc(n1);
+    if (!rc) rc = g->x_loff.alloc(n1 * 8);
+    if (!rc) rc = g->x_toff.alloc(n1 * 8);
+    if (!rc) rc = g->x_rows.alloc(n1 * 4);
+    if (!rc) rc = g->x_overflow.alloc(4);
+    if (rc) return rc;
+    PathsArgs A = paths_base(g);
+    CUDA_TRY(cudaMemsetAsync(A.x_vs, 0, n1, st));
+    CUDA_TRY(cudaMemsetAsync(A.x_loff, 0, n1 * 8, st));
+    CUDA_TRY(cudaMemsetAsync(A.x_toff, 0, n1 * 8, st));
+    CUDA_TRY(cudaMemsetAsync(A.x_overflow, 0, 4, st));
+    const unsigned grid = warp_grid(g, (n + 31) / 32);
+    node_links_kernel<false><<<grid, 256, 0, st>>>(A); g_launches++;
+    if ((rc = scan_i64(g, A.x_loff, A.x_loff, n + 1, st))) return rc;
+    template_kernel<false><<<grid, 256, 0, st>>>(A); g_launches++;
+    if ((rc = scan_i64(g, A.x_toff, A.x_toff, n + 1, st))) return rc;
+    int64_t NL = 0, TR = 0;
+    CUDA_TRY(cudaMemcpyAsync(&NL, A.x_loff + n, 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(&TR, A.x_toff + n, 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    // link records hold link and template offsets as int32
+    if (NL >= (1ll << 31) - 1 || TR >= (1ll << 31) - 1) return fail(ABB_ERR_CAPACITY, "exposure tables: %lld links, %lld template rows (int32 offsets)", (long long)NL, (long long)TR);
+    if (!rc) rc = g->x_link.alloc(static_cast<size_t>(NL) * 16);
+    if (!rc) rc = g->x_trow.alloc(static_cast<size_t>(TR) * 16);
+    if (!rc) rc = g->x_trel.alloc(static_cast<size_t>(TR) * 2);
+    if (rc) return rc;
+    A = paths_base(g);
+    template_kernel<true><<<grid, 256, 0, st>>>(A); g_launches++;
+    node_links_kernel<true><<<grid, 256, 0, st>>>(A); g_launches++;
+    unsigned overflow = 0;
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpyAsync(&overflow, A.x_overflow, 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (overflow) return fail(ABB_ERR_CAPACITY, "exposure tables: a finding has 2^31 or more exposure-path rows");
+    g->x_tables_ready = true;
+    return ABB_OK;
+}
+
+// Count pass of the exposure-path pipeline (paths.cuh): each finding's row count and links gathered from the exposure tables, then
+// one exclusive scan into io.f_off.  Once the tables exist this neither synchronises nor, for a batch no larger than an earlier
+// one, allocates.  `link_counts` also writes each finding's link count (pl_lcnt) for the host result.
+static int enqueue_paths_count(abb_graph *g, const abb_paths_io *io, cudaStream_t st, bool link_counts = false) {
+    NvtxRange nvtx_("paths: rows per finding");
     if (!io || io->n_findings < 0 || !io->f_off || (io->n_findings && !io->findings)) return fail(ABB_ERR_ARG, "bad paths io");
     if (io->n_findings >= (1ll << 31) - 2) return fail(ABB_ERR_ARG, "too many findings in one batch");
-    if (int rc = ensure_server_table(g, st)) return rc;
+    if (int rc = ensure_exposure_tables(g, st)) return rc;
     g->paths_args_valid = false;
-    const int64_t nf = io->n_findings, n = g->v.n;
-    PathsArgs A{};
-    A.g = g->v; A.io = *io; A.srv_cred = g->srv_cred.as<int32_t>(); A.srv_tool = g->srv_tool.as<int32_t>();
-    A.srv_roff = g->srv_roff.as<int64_t>(); A.srv_row = g->srv_row.as<int4>(); A.srv_rel = g->srv_rel.as<int8_t>();
-    int rc = ABB_OK;
-#define ENS(buf, bytes) if (!rc) rc = g->buf.ensure(static_cast<size_t>(bytes))
-    ENS(pl_cnt, (nf + 2) * 8); ENS(pl_off, (nf + 2) * 8); ENS(pl_need, n + 16); ENS(pl_ulist, (n + 2) * 4); ENS(pl_nu, 16);
-    ENS(pt_off_node, (n + 2) * 8); ENS(pt_cnt_node, (n + 2) * 4);
+    const int64_t nf = io->n_findings;
+    int rc = g->pl_cnt.ensure(static_cast<size_t>(nf + 1) * 8);
+    if (!rc) rc = g->pl_link.ensure(static_cast<size_t>(nf + 1) * 8);
+    if (!rc && link_counts) rc = g->pl_lcnt.ensure(static_cast<size_t>(nf + 1) * 8);
     if (rc) return rc;
-    A.link_cnt = g->pl_cnt.as<int64_t>(); A.link_off = g->pl_off.as<int64_t>(); A.need = g->pl_need.as<uint8_t>();
-    A.ulist = g->pl_ulist.as<int32_t>(); A.n_unique = g->pl_nu.as<unsigned long long>();
-    A.t_off_node = g->pt_off_node.as<int64_t>(); A.t_cnt_node = g->pt_cnt_node.as<int32_t>();
-    A.n_links = reinterpret_cast<const unsigned long long *>(A.link_off + nf);
-    CUDA_TRY(cudaMemsetAsync(A.link_cnt, 0, static_cast<size_t>(nf + 2) * 8, st));
-    if (nf) { links_kernel<false><<<warp_grid(g, (nf + 31) / 32), 256, 0, st>>>(A); g_launches++; }
-    if ((rc = scan_i64(g, A.link_cnt, A.link_off, nf + 1, st))) return rc;
-    int64_t NL = 0;
-    CUDA_TRY(cudaMemcpyAsync(&NL, A.link_off + nf, 8, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    const int64_t nu_max = std::min<int64_t>(NL, n);
-    ENS(pl_vs, (NL + 2) * 4); ENS(pl_rel, NL + 16); ENS(pl_f, (NL + 2) * 4); ENS(pl_rows, (NL + 2) * 8); ENS(pl_roff, (NL + 2) * 8); ENS(pl_toff, (NL + 2) * 8); ENS(pt_cnt, (nu_max + 2) * 8); ENS(pt_off, (nu_max + 2) * 8);
-    if (rc) return rc;
-    A.link_vs = g->pl_vs.as<int32_t>(); A.link_rel = g->pl_rel.as<int8_t>(); A.link_f = g->pl_f.as<int32_t>(); A.link_rows = g->pl_rows.as<int64_t>(); A.link_roff = g->pl_roff.as<int64_t>(); A.link_toff = g->pl_toff.as<int64_t>();
-    A.t_cnt = g->pt_cnt.as<int64_t>(); A.t_off = g->pt_off.as<int64_t>();
-    CUDA_TRY(cudaMemsetAsync(A.need, 0, static_cast<size_t>(n) + 16, st));
-    if (nf) { links_kernel<true><<<warp_grid(g, (nf + 31) / 32), 256, 0, st>>>(A); g_launches++; }
-    // unique vulnerable sources, node order
-    {
-        cub::CountingInputIterator<int32_t> iota(0);
-        size_t tmp = 0;
-        CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, tmp, iota, A.need, g->pl_ulist.as<int32_t>(), g->pl_nu.as<unsigned long long>(), static_cast<int>(n), st));
-        if ((rc = g->p_scan_tmp.ensure(tmp + 16))) return rc;
-        CUDA_TRY(cub::DeviceSelect::Flagged(g->p_scan_tmp.p, tmp, iota, A.need, g->pl_ulist.as<int32_t>(), g->pl_nu.as<unsigned long long>(), static_cast<int>(n), st));
-        g_launches++;
-    }
-    CUDA_TRY(cudaMemsetAsync(A.t_cnt, 0, static_cast<size_t>(nu_max + 2) * 8, st));
-    if (nu_max) { template_kernel<false><<<warp_grid(g, (nu_max + 31) / 32), 256, 0, st>>>(A); g_launches++; }
-    if ((rc = scan_i64(g, A.t_cnt, A.t_off, nu_max + 1, st))) return rc;
-    int64_t TR = 0;
-    CUDA_TRY(cudaMemcpyAsync(&TR, A.t_off + nu_max, 8, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    ENS(pt_row, (TR + 2) * 16); ENS(pt_rel, (TR + 2) * 2);
-    if (rc) return rc;
-#undef ENS
-    A.t_row = g->pt_row.as<int4>(); A.t_rel = g->pt_rel.as<int8_t>();
-    if (nu_max) { template_kernel<true><<<warp_grid(g, (nu_max + 31) / 32), 256, 0, st>>>(A); g_launches++; }
-    CUDA_TRY(cudaMemsetAsync(A.link_rows, 0, static_cast<size_t>(NL + 2) * 8, st));
-    if (NL) { link_rows_kernel<<<static_cast<unsigned>((NL + 255) / 256), 256, 0, st>>>(A); g_launches++; }
-    if ((rc = scan_i64(g, A.link_rows, A.link_roff, NL + 1, st))) return rc;
-    finding_offsets_kernel<<<static_cast<unsigned>((nf + 1 + 255) / 256), 256, 0, st>>>(A); g_launches++;
+    PathsArgs A = paths_base(g);
+    A.io = *io; A.f_cnt = g->pl_cnt.as<int64_t>(); A.f_link = g->pl_link.as<int2>(); A.f_lcnt = link_counts ? g->pl_lcnt.as<int64_t>() : nullptr;
+    finding_rows_kernel<<<static_cast<unsigned>((nf + 1 + 255) / 256), 256, 0, st>>>(A); g_launches++;
+    if ((rc = scan_i64(g, A.f_cnt, io->f_off, nf + 1, st))) return rc;
     CUDA_TRY(cudaGetLastError());
     g->paths_args = A;
     g->paths_args_valid = true;
-    g->paths_n_links = NL; g->paths_n_template_rows = TR;
     return ABB_OK;
 }
 
@@ -1572,12 +1592,55 @@ static int paths_run(abb_graph *g, const int32_t *h_findings, const int32_t *d_f
     abb_paths_io io{};
     io.n_findings = nf; io.findings = d_findings; io.f_off = g->p_off.as<int64_t>();
     CUDA_TRY(cudaEventRecord(g->ev[2], st));
-    if (int rc = enqueue_paths_count(g, &io, st)) return rc;
+    if (int rc = enqueue_paths_count(g, &io, st, true)) return rc;
+    // the batch's share of the exposure tables: its links (link counts scanned into link_off) and the templates of its distinct
+    // vulnerable sources, in node order
+    const PathsArgs A = g->paths_args;
+    const int64_t n = g->v.n;
+    int rc = g->pl_off.ensure(static_cast<size_t>(nf + 1) * 8);
+    if (rc) return rc;
+    int64_t *link_off = g->pl_off.as<int64_t>();
+    if ((rc = scan_i64(g, A.f_lcnt, link_off, nf + 1, st))) return rc;
+    int64_t NL = 0;
+    CUDA_TRY(cudaMemcpyAsync(&NL, link_off + nf, 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    const int64_t nu_max = std::min<int64_t>(NL, n);
+#define ENS(buf, bytes) if (!rc) rc = g->buf.ensure(static_cast<size_t>(bytes))
+    ENS(pl_vs, (NL + 2) * 4); ENS(pl_rel, NL + 16); ENS(pl_roff, (NL + 2) * 8); ENS(pl_toff, (NL + 2) * 8); ENS(pl_need, n + 16); ENS(pl_ulist, (n + 2) * 4);
+    ENS(pl_nu, 16); ENS(pt_cnt, (nu_max + 2) * 8); ENS(pt_off, (nu_max + 2) * 8); ENS(pt_off_node, (n + 2) * 8);
+    if (rc) return rc;
+    int32_t *link_vs = g->pl_vs.as<int32_t>(), *ulist = g->pl_ulist.as<int32_t>();
+    int8_t *link_rel = g->pl_rel.as<int8_t>();
+    int64_t *link_roff = g->pl_roff.as<int64_t>(), *link_toff = g->pl_toff.as<int64_t>(), *t_cnt = g->pt_cnt.as<int64_t>(), *t_off = g->pt_off.as<int64_t>();
+    uint8_t *need = g->pl_need.as<uint8_t>();
+    unsigned long long *nu = g->pl_nu.as<unsigned long long>();
+    CUDA_TRY(cudaMemsetAsync(need, 0, static_cast<size_t>(n) + 16, st));
+    batch_links_kernel<<<static_cast<unsigned>((nf + 1 + 255) / 256), 256, 0, st>>>(A, link_off, link_vs, link_rel, link_roff, need); g_launches++;
+    {
+        cub::CountingInputIterator<int32_t> iota(0);
+        size_t tmp = 0;
+        CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, tmp, iota, need, ulist, nu, static_cast<int>(n), st));
+        if ((rc = g->p_scan_tmp.ensure(tmp + 16))) return rc;
+        CUDA_TRY(cub::DeviceSelect::Flagged(g->p_scan_tmp.p, tmp, iota, need, ulist, nu, static_cast<int>(n), st));
+        g_launches++;
+    }
+    CUDA_TRY(cudaMemsetAsync(t_cnt, 0, static_cast<size_t>(nu_max + 2) * 8, st));
+    if (nu_max) { batch_template_counts_kernel<<<static_cast<unsigned>((nu_max + 255) / 256), 256, 0, st>>>(A, ulist, nu, t_cnt); g_launches++; }
+    if ((rc = scan_i64(g, t_cnt, t_off, nu_max + 1, st))) return rc;
+    int64_t TR = 0;
+    CUDA_TRY(cudaMemcpyAsync(&TR, t_off + nu_max, 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    ENS(pt_row, (TR + 2) * 16); ENS(pt_rel, (TR + 2) * 2);
+#undef ENS
+    if (rc) return rc;
+    int64_t *t_off_node = g->pt_off_node.as<int64_t>();
+    if (nu_max) { batch_templates_kernel<<<warp_grid(g, nu_max), 256, 0, st>>>(A, ulist, nu, t_off, t_off_node, g->pt_row.as<int4>(), g->pt_rel.as<int8_t>()); g_launches++; }
+    if (NL) { batch_link_toff_kernel<<<static_cast<unsigned>((NL + 255) / 256), 256, 0, st>>>(NL, link_vs, t_off_node, link_toff); g_launches++; }
+    CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaEventRecord(g->ev[3], st));
     g->paths_timed = true;
-    const PathsArgs &A = g->paths_args;
-    const size_t NL = static_cast<size_t>(g->paths_n_links), TR = static_cast<size_t>(g->paths_n_template_rows), n1 = static_cast<size_t>(nf) + 1;
-    r->n_links = g->paths_n_links; r->n_trows = g->paths_n_template_rows;
+    const size_t n1 = static_cast<size_t>(nf) + 1;
+    r->n_links = NL; r->n_trows = TR;
     bool ok = r->off.alloc(n1 * 8) && r->link_off.alloc(n1 * 8) && r->link_vs.alloc(NL * 4) && r->link_rel.alloc(NL) && r->link_roff.alloc((NL + 1) * 8) &&
               r->link_toff.alloc(NL * 8) && r->t_row.alloc(TR * 16) && r->t_rel.alloc(TR * 2);
     if (!ok) return fail(ABB_ERR_NOMEM, "pinned host allocation failed");
@@ -1586,8 +1649,8 @@ static int paths_run(abb_graph *g, const int32_t *h_findings, const int32_t *d_f
         if (e == cudaSuccess && bytes) e = cudaMemcpyAsync(dst.p, src, bytes, cudaMemcpyDeviceToHost, st);
         r->d2h += static_cast<int64_t>(bytes);
     };
-    d2h(r->off, io.f_off, n1 * 8); d2h(r->link_off, A.link_off, n1 * 8); d2h(r->link_vs, A.link_vs, NL * 4); d2h(r->link_rel, A.link_rel, NL);
-    d2h(r->link_roff, A.link_roff, (NL + 1) * 8); d2h(r->link_toff, A.link_toff, NL * 8); d2h(r->t_row, A.t_row, TR * 16); d2h(r->t_rel, A.t_rel, TR * 2);
+    d2h(r->off, io.f_off, n1 * 8); d2h(r->link_off, link_off, n1 * 8); d2h(r->link_vs, link_vs, NL * 4); d2h(r->link_rel, link_rel, NL);
+    d2h(r->link_roff, link_roff, (NL + 1) * 8); d2h(r->link_toff, link_toff, NL * 8); d2h(r->t_row, g->pt_row.p, TR * 16); d2h(r->t_rel, g->pt_rel.p, TR * 2);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail(ABB_ERR_CUDA, "paths D2H failed: %s", cudaGetErrorString(e));
     r->rows = r->off.as<int64_t>()[nf];
@@ -1671,7 +1734,7 @@ static int paths_rank(abb_graph *g, const int32_t *findings, int64_t n_findings,
     if (rc) return rc;
     PathsArgs A = g->paths_args;
     RankArgs RA{d_base.as<int32_t>(), d_tab.as<uint32_t>(), d_ncu.as<int32_t>(), d_ntu.as<int32_t>(), k1.as<unsigned long long>(), v1.as<uint32_t>(),
-                d_focus.as<uint8_t>(), io.findings, need};
+                d_focus.as<uint8_t>(), need};
     rank_keys_kernel<<<row_grid(g, rank_keys_kernel, g->rank_keys_grid), ROW_THREADS, 0, st>>>(A, RA); g_launches++;
     // sort input: every row (k1, v1), or the matched rows compacted into (k2, v2); the sorted pairs land in the other pair
     unsigned long long *key_in = k1.as<unsigned long long>(), *key_out = k2.as<unsigned long long>();
@@ -1753,8 +1816,8 @@ extern "C" int abb_exposure_host(abb_graph *g, const int32_t *findings, int64_t 
     auto now = [] { return std::chrono::steady_clock::now(); };
     auto ms = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) { return std::chrono::duration<double, std::milli>(b - a).count(); };
     const auto t0 = now();
-    // The exposure-path pipeline does not depend on the walk: it runs on its own stream, driven by a helper thread (its count pass
-    // synchronises that stream twice), while this thread stages and runs the walk.  The walk's node arena streams to the host over PCIe
+    // The exposure-path pipeline does not depend on the walk: it runs on its own stream, driven by a helper thread (sizing its
+    // factorised result synchronises that stream twice), while this thread stages and runs the walk.  The walk's node arena streams to the host over PCIe
     // as it is produced (zero-copy); the path pipeline's kernels and its factorised result copy fit inside that window.
     abb_paths_result *pr = nullptr;
     int prc = ABB_OK;

@@ -16,10 +16,12 @@
 // attached to vs shares.  The principals of a server depend only on the graph, so
 // they sit in a graph-constant server row table built once per graph
 // (server_rows_kernel); a template is the concatenation of its servers' table
-// rows.  Links and templates are built per call with one thread per finding /
-// vulnerable source in two passes (count, then fill at the scanned offsets) so
-// rows land in the reference's emission order; reverse rows longer than LONG_ROW
-// are handed to the whole warp.  The flat rows are then written row-parallel
+// rows.  Links and templates depend only on the graph too: they are built once per
+// graph for every finding node and every vulnerable source (ensure_exposure_tables)
+// with one thread per node in two passes (count, then fill at the scanned offsets)
+// so rows land in the reference's emission order; reverse rows longer than LONG_ROW
+// are handed to the whole warp.  A call then only gathers each finding's row count
+// and scans it (finding_rows_kernel), and writes the flat rows row-parallel
 // (for_each_row).  "Originals only" = entries without ABB_META_REVERSED_COPY: the
 // reference builds its incoming/outgoing maps from graph.edges, which never holds
 // the reversed copies of bidirectional edges (:698-702).
@@ -39,6 +41,10 @@ constexpr int REL_USES = 1, REL_DEPENDS_ON = 2, REL_PROVIDES_TOOL = 3, REL_EXPOS
 constexpr int ET_AGENT = 0, ET_SERVER = 1, ET_VULN = 8, ET_MISCONF = 9, ET_USER = 13, ET_SERVICE_ACCOUNT = 17;
 constexpr uint32_t LONG_ROW = 64;   // reverse rows longer than this are handled by the whole warp
 
+// A link of a finding node: x = vulnerable source, y = relationship of the pair (vs, finding), z = the link's first row within the
+// node's rows, w = first row of vs's template in t_row.
+using LinkRec = int4;
+
 struct PathsArgs {
     GraphView g;
     abb_paths_io io;
@@ -48,26 +54,19 @@ struct PathsArgs {
     const int64_t *srv_roff;    // [n_nodes+1] first table row of each node (only servers own rows, at least one each)
     const int4 *srv_row;        // [n_server_rows] agent, server, ncred, ntool
     const int8_t *srv_rel;      // [n_server_rows] relationship of the pair (agent, server)
-    // links: one per (finding, vulnerable source) in emission order
-    int64_t *link_cnt;          // [n_findings+1] links per finding (count pass), then scanned into link_off
-    int64_t *link_off;          // [n_findings+1]
-    int32_t *link_vs;           // [n_links]
-    int8_t *link_rel;           // [n_links] relationship of the pair (vs, finding)
-    int32_t *link_f;            // [n_links] finding index (position in io.findings) of the link
-    int64_t *link_rows;         // [n_links+1] rows per link, scanned into link_roff
-    int64_t *link_toff;         // [n_links] template offset of the link's vulnerable source
-    int64_t *link_roff;         // [n_links+1]
-    const unsigned long long *n_links;   // device scalar
-    // templates: the rows of one vulnerable source, shared by every finding attached to it
-    uint8_t *need;              // [n_nodes] vs is referenced by some link
-    const int32_t *ulist;       // [n_unique] vulnerable sources, node order
-    const unsigned long long *n_unique;  // device scalar
-    int64_t *t_cnt;             // [n_unique+1] rows per template, scanned into t_off
-    int64_t *t_off;             // [n_unique+1]
-    int64_t *t_off_node;        // [n_nodes] template offset by vs node
-    int32_t *t_cnt_node;        // [n_nodes] template length by vs node
+    // graph-constant exposure tables (ensure_exposure_tables): every finding node's links, every vulnerable source's template
+    uint8_t *x_vs;              // [n_nodes] 1 on a vulnerable source (a non-ghost source of an original VULNERABLE_TO entry into a finding)
+    int64_t *x_loff;            // [n_nodes+1] links of node u are x_link[x_loff[u] .. x_loff[u+1]) (counts, then scanned in place)
+    LinkRec *x_link;            // [n_links] in reverse-row order
+    int32_t *x_rows;            // [n_nodes] rows of node u (the sum of its links' template lengths; 0 for non-findings)
+    int64_t *x_toff;            // [n_nodes+1] template of node u is t_row[x_toff[u] .. x_toff[u+1]) (counts, then scanned in place)
     int4 *t_row;                // [n_template_rows] agent, server, ncred, ntool
     int8_t *t_rel;              // [n_template_rows*2] (agent,server) and (server,vs) relationships
+    unsigned *x_overflow;       // set when a node's rows do not fit the link record's int32
+    // per call
+    int64_t *f_cnt;             // [n_findings+1] rows of each finding, scanned into io.f_off
+    int2 *f_link;               // [n_findings] first link and link count of each finding
+    int64_t *f_lcnt;            // [n_findings+1] link counts (host-result path only, else nullptr)
 };
 
 // graph-constant table: credential / tool fan-out of every server (originals only, target must have a node record)
@@ -180,7 +179,7 @@ __global__ void __launch_bounds__(256) server_rows_kernel(const GraphView g, con
     }
 }
 
-// ---- pass A: links of every finding (VULNERABLE_TO originals whose source has a node record), in row order.
+// ---- exposure tables, links: every finding node's links (VULNERABLE_TO originals whose source has a node record), in row order.
 // The source behind reverse-row entry k of a finding, or -1; rvf = relationship of the pair (vs, finding), -3 = not the first
 // entry of the pair (looked up in the fill pass).
 __device__ __forceinline__ int32_t link_source(const GraphView &g, uint32_t k, int &rvf) {
@@ -192,63 +191,80 @@ __device__ __forceinline__ int32_t link_source(const GraphView &g, uint32_t k, i
     return v;
 }
 
-__device__ __forceinline__ void put_link(const PathsArgs &A, int64_t o, int32_t vs, int32_t f, int rvf, int64_t fi) {
+__device__ __forceinline__ int64_t template_rows(const PathsArgs &A, int32_t vs) { return A.x_toff[vs + 1] - A.x_toff[vs]; }
+
+// link record o of finding f: vs's template starts at x_toff[vs], the link's rows at `roff` within f's rows
+__device__ __forceinline__ void put_link(const PathsArgs &A, int64_t o, int32_t vs, int32_t f, int rvf, int64_t roff) {
     if (rvf == -3) rvf = first_rel_rev(A.g, vs, f);
-    A.link_vs[o] = vs; A.link_rel[o] = static_cast<int8_t>(rvf); A.link_f[o] = static_cast<int32_t>(fi);
-    A.need[vs] = 1;
+    A.x_link[o] = make_int4(vs, rvf, static_cast<int32_t>(roff), static_cast<int32_t>(A.x_toff[vs]));
 }
 
-// one thread per finding; a finding with a long reverse row is handed to the whole warp
+// Lane u owns node u; a finding with a long reverse row is handed to the whole warp.  COUNT writes the node's link count to
+// x_loff[u] (scanned in place afterwards) and flags its vulnerable sources in x_vs; FILL runs after the templates exist and writes
+// the link records from x_loff[u] and the node's row count.
 template <bool FILL>
-__global__ void __launch_bounds__(256) links_kernel(const PathsArgs A) {
+__global__ void __launch_bounds__(256) node_links_kernel(const PathsArgs A) {
     const GraphView &g = A.g;
     const int lane = threadIdx.x & 31;
     const int64_t warp = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = (static_cast<int64_t>(gridDim.x) * blockDim.x) >> 5;
-    const int64_t nf = A.io.n_findings;
-    for (int64_t base = warp * 32; base < nf; base += nwarps * 32) {
-        const int64_t fi = base + lane;
-        int32_t f = -1; uint32_t s0 = 0, e0 = 0;
-        if (fi < nf) {
-            f = __ldg(A.io.findings + fi);
-            bool ok = f >= 0 && f < g.n;
-            if (ok) { const uint8_t ft = __ldg(g.ntype + f); ok = ft == ET_VULN || ft == ET_MISCONF; }
-            if (ok) { s0 = __ldg(g.roff + f); e0 = __ldg(g.roff + f + 1); }
+    for (int64_t base = warp * 32; base < g.n; base += nwarps * 32) {
+        const int32_t u = static_cast<int32_t>(base + lane);
+        uint32_t s0 = 0, e0 = 0;
+        if (u < g.n) {
+            const uint8_t t = __ldg(g.ntype + u);
+            if (t == ET_VULN || t == ET_MISCONF) { s0 = __ldg(g.roff + u); e0 = __ldg(g.roff + u + 1); }
         }
         const bool is_long = e0 - s0 > LONG_ROW;
-        const int64_t o0 = (FILL && fi < nf) ? A.link_off[fi] : 0;
-        int64_t n = 0;
+        const int64_t o0 = (FILL && u < g.n) ? A.x_loff[u] : 0;
+        int64_t n = 0, rows = 0;
         if (!is_long) {
             for (uint32_t p = s0; p < e0; p++) {
                 int rvf;
                 const int32_t vs = link_source(g, p, rvf);
                 if (vs < 0) continue;
-                if (FILL) put_link(A, o0 + n, vs, f, rvf, fi);
+                if (FILL) { put_link(A, o0 + n, vs, u, rvf, rows); rows += template_rows(A, vs); }
+                else A.x_vs[vs] = 1;
                 n++;
             }
         }
         for (unsigned rem = __ballot_sync(FULL, is_long); rem; rem &= rem - 1) {
             const int src = __ffs(rem) - 1;
-            const int32_t lf = __shfl_sync(FULL, f, src);
+            const int32_t lu = __shfl_sync(FULL, u, src);
             const uint32_t ls0 = __shfl_sync(FULL, s0, src), le0 = __shfl_sync(FULL, e0, src);
-            const int64_t lo0 = __shfl_sync(FULL, o0, src), lfi = base + src;
-            int64_t ln = 0;
+            const int64_t lo0 = __shfl_sync(FULL, o0, src);
+            int64_t ln = 0, lrows = 0;
             for (uint32_t p = ls0; p < le0; p += 32) {
                 const uint32_t k = p + lane;
                 int rvf = -1;
                 const int32_t vs = k < le0 ? link_source(g, k, rvf) : -1;
                 const unsigned vm = __ballot_sync(FULL, vs >= 0);
-                if (FILL && vs >= 0) put_link(A, lo0 + ln + __popc(vm & lanemask_lt(lane)), vs, lf, rvf, lfi);
+                if (FILL) {
+                    const int64_t c = vs >= 0 ? template_rows(A, vs) : 0;
+                    int64_t inc = c;
+#pragma unroll
+                    for (int o = 1; o < 32; o <<= 1) { const int64_t v = __shfl_up_sync(FULL, inc, o); if (lane >= o) inc += v; }
+                    if (vs >= 0) put_link(A, lo0 + ln + __popc(vm & lanemask_lt(lane)), vs, lu, rvf, lrows + inc - c);
+                    lrows += __shfl_sync(FULL, inc, 31);
+                } else if (vs >= 0) {
+                    A.x_vs[vs] = 1;
+                }
                 ln += __popc(vm);
             }
-            if (lane == src) n = ln;
+            if (lane == src) { n = ln; rows = lrows; }
         }
-        if (!FILL && fi < nf) A.link_cnt[fi] = n;
+        if (u < g.n) {
+            if (!FILL) A.x_loff[u] = n;
+            else {
+                if (rows > 0x7FFFFFFF) atomicOr(A.x_overflow, 1u);
+                A.x_rows[u] = static_cast<int32_t>(rows);
+            }
+        }
     }
 }
 
-// ---- pass B: the template of each referenced vulnerable source (count, then fill): the server table's rows of vs itself when
-// it is a server, else of every server that DEPENDS_ON it, in reverse-row order.
+// ---- exposure tables, templates: the rows of every vulnerable source (count, then fill): the server table's rows of vs itself
+// when it is a server, else of every server that DEPENDS_ON it, in reverse-row order.
 // The server behind reverse-row entry k of a non-server vulnerable source, or -1; rsv as rvf above.
 __device__ __forceinline__ int32_t dependent_server(const GraphView &g, uint32_t k, int &rsv) {
     const uint32_t m = __ldg(g.rmeta + k);
@@ -270,21 +286,21 @@ __device__ __forceinline__ void copy_server_rows(const PathsArgs &A, int64_t row
     }
 }
 
-// one thread per vulnerable source; one with a long reverse row is handed to the whole warp
+// Lane u owns node u when it is a vulnerable source; one with a long reverse row is handed to the whole warp.  COUNT writes the
+// template length to x_toff[u] (0 for other nodes; scanned in place afterwards), FILL writes the rows from x_toff[u].
 template <bool FILL>
 __global__ void __launch_bounds__(256) template_kernel(const PathsArgs A) {
     const GraphView &g = A.g;
     const int lane = threadIdx.x & 31;
     const int64_t warp = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = (static_cast<int64_t>(gridDim.x) * blockDim.x) >> 5;
-    const int64_t nu = static_cast<int64_t>(*A.n_unique);
-    for (int64_t base = warp * 32; base < nu; base += nwarps * 32) {
-        const int64_t ui = base + lane;
+    for (int64_t base = warp * 32; base < g.n; base += nwarps * 32) {
+        const int64_t u = base + lane;
         int32_t vs = -1; uint32_t s2 = 0, e2 = 0; bool is_long = false;
         int64_t row = 0, n = 0;
-        if (ui < nu) {
-            vs = __ldg(A.ulist + ui);
-            if (FILL) row = A.t_off[ui];
+        if (u < g.n && A.x_vs[u]) {
+            vs = static_cast<int32_t>(u);
+            if (FILL) row = A.x_toff[vs];
             if (__ldg(g.ntype + vs) == ET_SERVER) {
                 n = server_rows(A, vs);
                 if (FILL) copy_server_rows(A, row, vs, vs, -2);
@@ -321,30 +337,82 @@ __global__ void __launch_bounds__(256) template_kernel(const PathsArgs A) {
             }
             if (lane == src) n = ln;
         }
-        if (ui < nu) {
-            if (!FILL) { A.t_cnt[ui] = n; A.t_cnt_node[vs] = static_cast<int32_t>(n); }
-            else A.t_off_node[vs] = row;
-        }
+        if (!FILL && u < g.n) A.x_toff[u] = n;
     }
 }
 
-__global__ void link_rows_kernel(const PathsArgs A) {
+// ---- per call: each finding's rows and links from the tables.  Ids that are out of range or not findings have none; thread
+// n_findings writes the 0 that the exclusive scan turns into the total.
+__global__ void finding_rows_kernel(const PathsArgs A) {
+    const int64_t fi = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x, nf = A.io.n_findings;
+    if (fi > nf) return;
+    int64_t rows = 0;
+    int2 fl = make_int2(0, 0);
+    if (fi < nf) {
+        const int32_t f = __ldg(A.io.findings + fi);
+        if (f >= 0 && f < A.g.n) {
+            const int64_t l0 = __ldg(A.x_loff + f);
+            fl = make_int2(static_cast<int32_t>(l0), static_cast<int32_t>(__ldg(A.x_loff + f + 1) - l0));
+            rows = __ldg(A.x_rows + f);
+        }
+        A.f_link[fi] = fl;
+    }
+    A.f_cnt[fi] = rows;
+    if (A.f_lcnt) A.f_lcnt[fi] = fl.y;
+}
+
+// ---- host result (abb_paths_host / abb_exposure_host): the batch's links with their flat rows, and its vulnerable sources flagged
+__global__ void batch_links_kernel(const PathsArgs A, const int64_t *link_off, int32_t *link_vs, int8_t *link_rel, int64_t *link_roff, uint8_t *need) {
+    const int64_t fi = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x, nf = A.io.n_findings;
+    if (fi == nf) link_roff[link_off[nf]] = A.io.f_off[nf];
+    if (fi >= nf) return;
+    const int2 fl = A.f_link[fi];
+    const int64_t o0 = link_off[fi], r0 = A.io.f_off[fi];
+    for (int k = 0; k < fl.y; k++) {
+        const LinkRec l = __ldg(A.x_link + fl.x + k);
+        link_vs[o0 + k] = l.x; link_rel[o0 + k] = static_cast<int8_t>(l.y); link_roff[o0 + k] = r0 + l.z;
+        need[l.x] = 1;
+    }
+}
+
+// template lengths of the batch's distinct vulnerable sources (ulist, node order)
+__global__ void batch_template_counts_kernel(const PathsArgs A, const int32_t *ulist, const unsigned long long *n_unique, int64_t *t_cnt) {
+    const int64_t ui = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (ui < static_cast<int64_t>(*n_unique)) t_cnt[ui] = template_rows(A, ulist[ui]);
+}
+
+// one warp per distinct vulnerable source: its template rows to the batch's offset t_off[ui]
+__global__ void batch_templates_kernel(const PathsArgs A, const int32_t *ulist, const unsigned long long *n_unique, const int64_t *t_off,
+                                       int64_t *t_off_node, int4 *t_row, int8_t *t_rel) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warp = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+    const int64_t nwarps = (static_cast<int64_t>(gridDim.x) * blockDim.x) >> 5;
+    const int64_t nu = static_cast<int64_t>(*n_unique);
+    for (int64_t ui = warp; ui < nu; ui += nwarps) {
+        const int32_t vs = ulist[ui];
+        const int64_t s = A.x_toff[vs], e = A.x_toff[vs + 1], o = t_off[ui];
+        for (int64_t k = lane; k < e - s; k += 32) {
+            t_row[o + k] = A.t_row[s + k];
+            reinterpret_cast<uint16_t *>(t_rel)[o + k] = reinterpret_cast<const uint16_t *>(A.t_rel)[s + k];
+        }
+        if (lane == 0) t_off_node[vs] = o;
+    }
+}
+
+__global__ void batch_link_toff_kernel(int64_t n_links, const int32_t *link_vs, const int64_t *t_off_node, int64_t *link_toff) {
     const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-    if (i < static_cast<int64_t>(*A.n_links)) { const int32_t vs = A.link_vs[i]; A.link_rows[i] = A.t_cnt_node[vs]; A.link_toff[i] = A.t_off_node[vs]; }
+    if (i < n_links) link_toff[i] = t_off_node[link_vs[i]];
 }
 
-__global__ void finding_offsets_kernel(const PathsArgs A) {
-    const int64_t fi = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-    if (fi <= A.io.n_findings) A.io.f_off[fi] = A.link_roff[A.link_off[fi]];
-}
-
-// ---- pass C: every link copies its vulnerable source's template, substituting the finding.
+// ---- replicate: every finding copies its links' templates, substituting the finding.
 // Row-parallel: the flat rows [0, R) are cut into tiles of ROW_TILE, and a block takes a contiguous run of tiles.  Warp w of the
 // block takes ROW_ITEMS * 32 consecutive rows of a tile, 32 at a time, so each output stream is written in whole coalesced lines.
-// The links of a tile are found in the block's shared copy of the link_roff window that starts at the tile's first link (ROW_WIN
-// links, stored relative to the tile's first row).  A warp carries its current link from step to step: a lane searches only when
-// its row lies past that link's end, which in long links (almost every row) is one shared-memory compare.  A tile that spans
-// more links than the window holds (a run of zero-row links) searches the rest in global memory.
+// The findings of a tile are found in the block's shared copy of the io.f_off window that starts at the tile's first finding
+// (ROW_WIN findings, stored relative to the tile's first row).  A warp carries its current finding from step to step: a lane
+// searches only when its row lies past that finding's end, which in long findings (most rows) is one shared-memory compare.  A
+// tile that spans more findings than the window holds (a run of zero-row findings) searches the rest in global memory.  Each lane
+// keeps its last row's finding, first link and template, so a row of the same finding with one link (most of them) loads nothing
+// but its template row; a finding with several links searches their first rows.
 // The tile size and 6 resident blocks per SM for replicate_kernel are what measured fastest at L on the H100: a block's two
 // barriers and window load per tile are exposed latency, which larger tiles and more resident warps hide (unrolling steps to
 // keep more loads in flight per warp cost registers, hence occupancy, and did not help).
@@ -357,29 +425,50 @@ __device__ __forceinline__ I last_le(const T *roff, I lo, I hi, T r) {
     return lo;
 }
 
-// Visits every flat row once as fn.store(row, fn.load(row, link)).  Every thread of the block must call it (ROW_THREADS per block).
+// the link holding row q of a finding whose links are x_link[fl.x .. fl.x + fl.y), fl.y >= 1
+__device__ __forceinline__ LinkRec link_of_row(const PathsArgs &A, int2 fl, int32_t q) {
+    int32_t lo = fl.x, hi = fl.x + fl.y;
+    const int32_t *first_row = reinterpret_cast<const int32_t *>(A.x_link) + 2;   // .z of record k at 4 * k
+    while (hi - lo > 1) { const int32_t mid = (lo + hi) >> 1; if (__ldg(first_row + 4 * static_cast<int64_t>(mid)) <= q) lo = mid; else hi = mid; }
+    return __ldg(A.x_link + lo);
+}
+
+// what locates one flat row: its template row, vulnerable source, finding node, (vs, finding) relationship and finding index
+struct RowRef {
+    int64_t t;
+    int32_t vs, f, rel;
+    int64_t fi;
+};
+
+// Visits every flat row once as fn(row, RowRef).  Every thread of the block must call it (ROW_THREADS per block).
 template <class Fn>
 __device__ __forceinline__ void for_each_row(const PathsArgs &A, const Fn &fn) {
-    __shared__ int32_t s_roff[ROW_WIN + 1];   // link_roff[l0 + i] - r0, clamped to [-1, ROW_TILE + 1]: exact for every comparison with a row of the tile
+    __shared__ int32_t s_roff[ROW_WIN + 1];   // f_off[l0 + i] - r0, clamped to [-1, ROW_TILE + 1]: exact for every comparison with a row of the tile
     __shared__ int64_t s_l0;
     const int lane = threadIdx.x & 31, w0 = (threadIdx.x >> 5) * ROW_ITEMS * 32;
-    const int64_t NL = static_cast<int64_t>(*A.n_links), R = A.link_roff[NL];
+    const int64_t *foff = A.io.f_off;
+    const int64_t NF = A.io.n_findings, R = foff[NF];
     const int64_t ntiles = (R + ROW_TILE - 1) / ROW_TILE, per = (ntiles + gridDim.x - 1) / gridDim.x;
     const int64_t tb = blockIdx.x * per, te = min(ntiles, tb + per);
     if (tb >= te) return;
-    if (threadIdx.x == 0) s_l0 = last_le(A.link_roff, int64_t{0}, NL, tb * ROW_TILE);
+    if (threadIdx.x == 0) s_l0 = last_le(foff, int64_t{0}, NF, tb * ROW_TILE);
+    // this lane's last finding: index, node, whether it has several links, else its link's source, relationship and the template
+    // row of flat row 0 (a row's template row is ct0 + row)
+    int64_t ct0 = 0;
+    int32_t cfi = -1, cf = 0, cvs = 0, crel = 0;
+    bool cmulti = false;
     for (int64_t tile = tb; tile < te; tile++) {
         __syncthreads();
         const int64_t l0 = s_l0, r0 = tile * ROW_TILE;
         const int n = static_cast<int>(min(static_cast<int64_t>(ROW_TILE), R - r0));   // rows of this tile
-        const int nw = static_cast<int>(min(static_cast<int64_t>(ROW_WIN), NL - l0));  // window: links l0 .. l0+nw-1, bounds s_roff[0..nw]
+        const int nw = static_cast<int>(min(static_cast<int64_t>(ROW_WIN), NF - l0));  // window: findings l0 .. l0+nw-1, bounds s_roff[0..nw]
         for (int i = threadIdx.x; i <= nw; i += ROW_THREADS) {
-            const int64_t d = A.link_roff[l0 + i] - r0;
+            const int64_t d = foff[l0 + i] - r0;
             s_roff[i] = d < 0 ? -1 : static_cast<int32_t>(min(d, static_cast<int64_t>(ROW_TILE + 1)));
         }
         __syncthreads();
-        const int wend = s_roff[nw];   // tile rows below this lie in the window's links
-        int j = 0;                     // warp-uniform: window link of the warp's last row so far
+        const int wend = s_roff[nw];   // tile rows below this lie in the window's findings
+        int j = 0;                     // warp-uniform: window finding of the warp's last row so far
         for (int it = 0; it < ROW_ITEMS && w0 + it * 32 < n; it++) {
             const int k = w0 + it * 32 + lane;
             int jl = j;
@@ -389,14 +478,26 @@ __device__ __forceinline__ void for_each_row(const PathsArgs &A, const Fn &fn) {
                     if (s_roff[jl + 1] <= k) jl = last_le(s_roff, jl + 1, nw, static_cast<int32_t>(k));
                     l = l0 + jl;
                 } else {
-                    l = last_le(A.link_roff, l0 + nw, NL, r0 + k);
+                    l = last_le(foff, l0 + nw, NF, r0 + k);
                 }
-                fn.store(r0 + k, fn.load(r0 + k, l));
+                if (static_cast<int32_t>(l) != cfi) {
+                    cfi = static_cast<int32_t>(l); cf = __ldg(A.io.findings + l);
+                    const int2 fl = __ldg(A.f_link + l);
+                    cmulti = fl.y > 1;
+                    if (!cmulti) { const LinkRec rec = __ldg(A.x_link + fl.x); cvs = rec.x; crel = rec.y; ct0 = rec.w - rec.z - __ldg(foff + l); }
+                }
+                if (!cmulti) {
+                    fn(r0 + k, RowRef{ct0 + r0 + k, cvs, cf, crel, l});
+                } else {
+                    const int32_t q = static_cast<int32_t>(r0 + k - __ldg(foff + l));
+                    const LinkRec rec = link_of_row(A, __ldg(A.f_link + l), q);
+                    fn(r0 + k, RowRef{rec.w + static_cast<int64_t>(q - rec.z), rec.x, cf, rec.y, l});
+                }
             }
             j = __shfl_sync(FULL, jl, 31);   // rows ascend with the lane; a partial step is the tile's last
         }
         if (threadIdx.x == 0 && r0 + ROW_TILE < R)
-            s_l0 = ROW_TILE < wend ? l0 + last_le(s_roff, 0, nw, static_cast<int32_t>(ROW_TILE)) : last_le(A.link_roff, l0 + nw, NL, r0 + ROW_TILE);
+            s_l0 = ROW_TILE < wend ? l0 + last_le(s_roff, 0, nw, static_cast<int32_t>(ROW_TILE)) : last_le(foff, l0 + nw, NF, r0 + ROW_TILE);
     }
 }
 
@@ -407,12 +508,9 @@ struct RowValue {
     int32_t vs, f, rel;
 };
 
-__device__ __forceinline__ RowValue row_value(const PathsArgs &A, int64_t t, int32_t vs, int32_t f, int rel) {
-    return RowValue{__ldg(A.t_row + t), __ldg(reinterpret_cast<const uint16_t *>(A.t_rel) + t), vs, f, rel};
+__device__ __forceinline__ RowValue row_value(const PathsArgs &A, const RowRef &x) {
+    return RowValue{__ldg(A.t_row + x.t), __ldg(reinterpret_cast<const uint16_t *>(A.t_rel) + x.t), x.vs, x.f, x.rel};
 }
-
-// template row of flat row r of link l
-__device__ __forceinline__ int64_t template_row(const PathsArgs &A, int64_t r, int64_t l) { return __ldg(A.link_toff + l) + (r - __ldg(A.link_roff + l)); }
 
 __device__ __forceinline__ void emit_row(const PathsArgs &A, int64_t out, const RowValue &v) {
     const int32_t srv = v.tr.y;
@@ -428,11 +526,7 @@ __device__ __forceinline__ void emit_row(const PathsArgs &A, int64_t out, const 
 
 struct ReplicateRows {
     const PathsArgs &A;
-    using Value = RowValue;
-    __device__ __forceinline__ Value load(int64_t r, int64_t l) const {
-        return row_value(A, template_row(A, r, l), __ldg(A.link_vs + l), __ldg(A.io.findings + __ldg(A.link_f + l)), __ldg(A.link_rel + l));
-    }
-    __device__ __forceinline__ void store(int64_t r, const Value &v) const { emit_row(A, r, v); }
+    __device__ __forceinline__ void operator()(int64_t r, const RowRef &x) const { emit_row(A, r, row_value(A, x)); }
 };
 
 __global__ void __launch_bounds__(ROW_THREADS, 6) replicate_kernel(const PathsArgs A) { for_each_row(A, ReplicateRows{A}); }
@@ -465,8 +559,7 @@ struct RankArgs {
     unsigned long long *keys;     // [n_rows] complemented sort key
     uint32_t *rows;               // [n_rows] row index, ~0u when the row misses the focus
     const uint8_t *focus;         // [n_nodes] focus bits of every node, or nullptr: every row matches
-    const int32_t *findings;      // [n_findings] finding node of each finding index (focused pass only)
-    uint32_t need;                // categories every matching row must satisfy
+    uint32_t need;               // categories every matching row must satisfy
 };
 
 constexpr uint32_t ROW_UNMATCHED = 0xFFFFFFFFu;
@@ -481,17 +574,14 @@ __device__ __forceinline__ bool row_matches(const RankArgs &R, int32_t agent, in
 struct RankRows {
     const PathsArgs &A;
     const RankArgs &R;
-    struct Value { int4 tr; int32_t fi, vs; };
-    __device__ __forceinline__ Value load(int64_t r, int64_t l) const {
-        return Value{__ldg(A.t_row + template_row(A, r, l)), __ldg(A.link_f + l), __ldg(A.link_vs + l)};
-    }
-    __device__ __forceinline__ void store(int64_t r, const Value &v) const {
-        const int nc = v.tr.z < 4 ? v.tr.z : 4, nt = v.tr.w < 14 ? v.tr.w : 14;
-        const unsigned long long rr = R.risk_rank[(static_cast<int64_t>(R.base_id[v.fi]) * 5 + nc) * 15 + nt];
-        const unsigned long long nh = (v.vs != v.tr.y) ? 4ull : 3ull;
-        const unsigned long long cu = static_cast<unsigned long long>(min(R.ncu[v.tr.y], 0x3FFFF)), tu = static_cast<unsigned long long>(min(R.ntu[v.tr.y], 0x3FFFF));
+    __device__ __forceinline__ void operator()(int64_t r, const RowRef &x) const {
+        const int4 tr = __ldg(A.t_row + x.t);
+        const int nc = tr.z < 4 ? tr.z : 4, nt = tr.w < 14 ? tr.w : 14;
+        const unsigned long long rr = R.risk_rank[(static_cast<int64_t>(R.base_id[x.fi]) * 5 + nc) * 15 + nt];
+        const unsigned long long nh = (x.vs != tr.y) ? 4ull : 3ull;
+        const unsigned long long cu = static_cast<unsigned long long>(min(R.ncu[tr.y], 0x3FFFF)), tu = static_cast<unsigned long long>(min(R.ntu[tr.y], 0x3FFFF));
         R.keys[r] = ~((rr << 40) | (nh << 36) | (cu << 18) | tu);
-        const bool hit = !R.focus || row_matches(R, v.tr.x, v.tr.y, v.vs, __ldg(R.findings + v.fi));
+        const bool hit = !R.focus || row_matches(R, tr.x, tr.y, x.vs, x.f);
         R.rows[r] = hit ? static_cast<uint32_t>(r) : ROW_UNMATCHED;
     }
 };
@@ -515,16 +605,11 @@ __global__ void rank_gather_kernel(const PathsArgs A, const RankArgs R, const ui
     const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (i >= count) return;
     const int64_t row = sorted_rows[first + i];
-    // finding = last f with f_off[f] <= row; link = last l in the finding with link_roff[l] <= row
-    int64_t lo = 0, hi = A.io.n_findings;
-    while (hi - lo > 1) { const int64_t mid = (lo + hi) >> 1; if (A.io.f_off[mid] <= row) lo = mid; else hi = mid; }
-    const int64_t fi = lo;
-    int64_t a = A.link_off[fi], b = A.link_off[fi + 1];
-    while (b - a > 1) { const int64_t mid = (a + b) >> 1; if (A.link_roff[mid] <= row) a = mid; else b = mid; }
-    const int64_t l = a;
-    const int32_t vs = A.link_vs[l];
-    const int64_t t = A.t_off_node[vs] + (row - A.link_roff[l]);
-    const RowValue v = row_value(A, t, vs, A.io.findings[fi], A.link_rel[l]);
+    // finding = last f with f_off[f] <= row, then the finding's link that holds the row
+    const int64_t fi = last_le(A.io.f_off, int64_t{0}, A.io.n_findings, row);
+    const int32_t q = static_cast<int32_t>(row - A.io.f_off[fi]);
+    const LinkRec l = link_of_row(A, A.f_link[fi], q);
+    const RowValue v = row_value(A, RowRef{l.w + static_cast<int64_t>(q - l.z), l.x, A.io.findings[fi], l.y, fi});
     emit_row(A, i, v);
     const int4 tr = v.tr;
     const int nc = tr.z < 4 ? tr.z : 4, nt = tr.w < 14 ? tr.w : 14;
