@@ -59,15 +59,17 @@ __device__ double pairwise_sum(const double *a, int64_t n) {
 
 // ---------------------------------------------------------------- PageRank (_pagerank_scipy)
 // scipy's row sums S = A.sum(axis=1) are np.add.reduceat over each row's weights in ascending column order: w0 + pw(w1..).
-// inv = 1/S (0 for a dangling row, flagged).
+// inv = 1/S where S != 0, else 0; a row is dangling when inv == 0 (is_dangling = S == 0 after S[S != 0] = 1/S), so a sum that
+// overflowed to +-inf is dangling too.
 __global__ void pr_rowsum_kernel(int32_t n, const uint32_t *off, const double *w_sorted, double *inv, uint8_t *dangling) {
     for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
         const int64_t a = off[i], k = static_cast<int64_t>(off[i + 1]) - a;
         double s = 0.0;
         if (k == 1) s = w_sorted[a];
         else if (k > 1) s = __dadd_rn(w_sorted[a], pairwise_sum(w_sorted + a + 1, k - 1));
-        inv[i] = s != 0.0 ? __ddiv_rn(1.0, s) : 0.0;
-        dangling[i] = s == 0.0;
+        const double r = s != 0.0 ? __ddiv_rn(1.0, s) : 0.0;
+        inv[i] = r;
+        dangling[i] = r == 0.0;
     }
 }
 
@@ -77,13 +79,16 @@ __global__ void pr_edge_weight_kernel(int64_t m, const uint32_t *feid, const dou
         w_edge[feid[e] >> 1] = w[e];
 }
 
-// reverse entry r of row k = in-edge (j -> k): key j, value A[j,k] = inv[j] * w (scipy's Q @ A)
+// reverse entry r of row k = in-edge (j -> k): key j, value A[j,k] = inv[j] * w (scipy's Q @ A).  Q = dia_array((1/S, 0)) drops
+// a zero diagonal entry, so a row with inv 0 has no entries in Q @ A; its value is 0.0, which leaves a finite sum as it was
+// (never 0 * inf = NaN).
 __global__ void pr_rev_values_kernel(int64_t m, const int32_t *rnbr, const uint32_t *reid, const double *inv, const double *w_edge, int32_t *key,
                                      double *val) {
     for (int64_t r = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; r < m; r += static_cast<int64_t>(gridDim.x) * blockDim.x) {
         const int32_t j = rnbr[r];
+        const double ij = inv[j];
         key[r] = j;
-        val[r] = __dmul_rn(inv[j], w_edge[reid[r] >> 1]);
+        val[r] = ij == 0.0 ? 0.0 : __dmul_rn(ij, w_edge[reid[r] >> 1]);
     }
 }
 

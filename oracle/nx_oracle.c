@@ -67,7 +67,9 @@ int nxo_pagerank(int32_t n, const int64_t *foff, const int32_t *fnbr, const doub
         else if (k > 1) s = ws[a] + pairwise(ws + a + 1, k - 1);
         inv[i] = s != 0.0 ? 1.0 / s : 0.0;
     }
-    /* x @ A: y[k] = sum over j ascending of (inv[j] * w[j,k]) * x[j], from 0.0 — built as column lists in ascending j */
+    /* x @ A: y[k] = sum over j ascending of (inv[j] * w[j,k]) * x[j], from 0.0 — built as column lists in ascending j.  scipy's
+     * Q = dia_array((1/S, 0)) drops a zero diagonal entry, so a row with inv 0 (dangling, or a sum that overflowed to inf) has
+     * no entries in Q @ A: it contributes 0.0 (adding +-0 leaves a finite y as it was), never inv * w = 0 * inf = NaN. */
     int64_t *coff = calloc((size_t)n + 1, sizeof(int64_t));
     for (int64_t e = 0; e < m; e++) coff[row[e].col + 1]++;
     for (int32_t k = 0; k < n; k++) coff[k + 1] += coff[k];
@@ -79,7 +81,7 @@ int nxo_pagerank(int32_t n, const int64_t *foff, const int32_t *fnbr, const doub
         for (int64_t e = foff[j]; e < foff[j + 1]; e++) {
             const int64_t at = fill[row[e].col]++;
             csrc[at] = j;
-            cval[at] = inv[j] * row[e].w;
+            cval[at] = inv[j] == 0.0 ? 0.0 : inv[j] * row[e].w;
         }
     double *x = malloc(sizeof(double) * (size_t)n), *xn = malloc(sizeof(double) * (size_t)n), *diff = malloc(sizeof(double) * (size_t)n);
     const double p = 1.0 / n;
@@ -117,7 +119,9 @@ static int64_t brandes_one(int32_t n, const int64_t *foff, const int32_t *fnbr, 
         }
         scanned += foff[v + 1] - foff[v];
     }
-    for (int64_t i = tail - 1; i >= 0; i--) {
+    /* down to queue position 1: the source (position 0) has no predecessor one level up, and at dist[s] - 1 == -1 its scan would
+     * match every unreached in-neighbour, adding sigma 0 * coeff — NaN once path counts overflow to inf */
+    for (int64_t i = tail - 1; i >= 1; i--) {
         const int32_t w = queue[i];
         const double coeff = (1.0 + delta[w]) / sigma[w];
         for (int64_t e = roff[w]; e < roff[w + 1]; e++) {
