@@ -203,6 +203,8 @@ EXPORTS = {
     "abb_union_result_w1": (vp, [vp]),
     "abb_union_result_ms": (C.c_double, [vp]),
     "abb_union_result_free": (None, [vp]),
+    "abb_clusters_build_host": (C.c_int, [vp, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "abb_clusters_fetch_host": (C.c_int, [vp, i64, vp, vp, vp, vp]),
 }
 
 _lock = threading.Lock()

@@ -30,6 +30,7 @@
 #include "centrality.cuh"
 #include "nxcentral.cuh"
 #include "lateral.cuh"
+#include "clusters.cuh"
 #include "walk.cuh"
 #include "walkb.cuh"
 
@@ -282,6 +283,11 @@ struct abb_graph {
     DevBuf cx_bcnt, cx_cnt, cx_start, cx_src;
     cudaEvent_t cx_staged = nullptr;
     cudaEvent_t cx_ev[4] = {nullptr, nullptr, nullptr, nullptr};
+    // graph-constant semantic-cluster tables (clusters_host.inl): each cluster's members in id order, its (cluster << 5 | rel) pairs and
+    // their counts; host copies of both segment offsets [K+1].  cl_k = -1 until built.
+    DevBuf cl_members, cl_rel_key, cl_rel_cnt;
+    std::vector<int64_t> cl_mem_off, cl_rel_off;
+    int64_t cl_k = -1;
     // graph arrays of an uploaded graph (an adopted graph's belong to the caller)
     std::vector<DevBuf> owned_arrays;
 
@@ -1955,3 +1961,4 @@ extern "C" int abb_finding_context_host(abb_graph *g, int32_t max_depth, const i
 #include "centrality_host.inl"
 #include "nxcentral_host.inl"
 #include "lateral_host.inl"
+#include "clusters_host.inl"

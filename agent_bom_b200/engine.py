@@ -546,6 +546,35 @@ class DeviceGraph:
             _lib.check(_lib.load().abb_pagerank_host(h, w.ctypes.data, out.ctypes.data, C.byref(iters)))
         return out, int(iters.value)
 
+    def build_clusters(self, k: int, codes, level, risk, etype) -> dict[str, np.ndarray]:
+        """Build the graph's semantic-cluster tables (``abb_clusters_build_host``), replacing earlier ones, and return the per-cluster
+        summaries: ``count``, ``max_risk``, ``hist`` [k, 5], ``type_mask`` and ``rel_nnz``.  ``codes``: int32 [n_nodes, 2]
+        (-1 = none); ``level`` / ``risk`` / ``etype``: per node."""
+        n = self.n_nodes
+        codes = np.ascontiguousarray(codes, dtype=np.int32).reshape(n, 2)
+        level = np.ascontiguousarray(level, dtype=np.uint8)
+        risk = np.ascontiguousarray(risk, dtype=np.float64)
+        etype = np.ascontiguousarray(etype, dtype=np.uint8)
+        if level.shape != (n,) or risk.shape != (n,) or etype.shape != (n,):
+            raise ValueError("cluster inputs need one entry per node")
+        out = {"count": np.zeros(k, np.int64), "max_risk": np.zeros(k, np.float64), "hist": np.zeros((k, 5), np.int64),
+               "type_mask": np.zeros(k, np.uint64), "rel_nnz": np.zeros(k, np.int64)}
+        with self._use() as h:
+            _lib.check(_lib.load().abb_clusters_build_host(h, k, codes.ctypes.data, level.ctypes.data, risk.ctypes.data, etype.ctypes.data,
+                                                           *(out[f].ctypes.data for f in ("count", "max_risk", "hist", "type_mask", "rel_nnz"))))
+        return out
+
+    def fetch_clusters(self, sel, n_members: int, n_pairs: int) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """Members (node indices in id order) and (relationship code, edge count) pairs of the selected clusters, concatenated in
+        selection order (``abb_clusters_fetch_host``); the caller sizes the outputs from the build's ``count`` and ``rel_nnz``."""
+        sel = _i32(sel)
+        members = np.empty(n_members, np.int32)
+        rel = np.empty(n_pairs, np.uint8)
+        cnt = np.empty(n_pairs, np.int64)
+        with self._use() as h:
+            _lib.check(_lib.load().abb_clusters_fetch_host(h, sel.shape[0], sel.ctypes.data, members.ctypes.data, rel.ctypes.data, cnt.ctypes.data))
+        return members, rel, cnt
+
     def betweenness(self) -> np.ndarray:
         """``nx.betweenness_centrality`` of the graph as a DiGraph (``abb_betweenness_host``): f64 per node."""
         out = np.zeros(self.n_nodes, dtype=np.float64)

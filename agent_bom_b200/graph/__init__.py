@@ -7,6 +7,7 @@ Mirrors ``/root/reference/src/agent_bom/graph/__init__.py:8-100`` for the names 
 """
 
 from .builder import build_unified_graph_from_report
+from .clusters import SEMANTIC_CLUSTER_KINDS, SemanticCluster, SemanticClusterExpansion, semantic_cluster_stats, semantic_clusters, semantic_clusters_view
 from .container import UnifiedGraph
 from .dependency_reach import PackageReachability, ReachabilityReport, VulnerabilityReachability, compute_dependency_reach
 from .envelope import EdgeIndex, exposure_path_for_attack_path, mcp_exposure_path_payload, serialize_attack_path, serialize_attack_paths
@@ -22,4 +23,5 @@ __all__ = [
     "UnifiedEdge", "UnifiedGraph", "UnifiedNode", "VulnerabilityReachability", "build_unified_graph_from_report", "compute_dependency_reach", "derived_attack_paths", "exposure_path_rows",
     "materialize_attack_paths", "node_risk_100", "ranked_attack_paths", "EdgeIndex", "exposure_path_for_attack_path", "mcp_exposure_path_payload",
     "serialize_attack_path", "serialize_attack_paths", "fix_first_view", "iter_ocsf_events", "ocsf_event",
+    "SEMANTIC_CLUSTER_KINDS", "SemanticCluster", "SemanticClusterExpansion", "semantic_cluster_stats", "semantic_clusters", "semantic_clusters_view",
 ]

@@ -70,6 +70,7 @@ class UnifiedGraph:
         self._rank_inputs = None
         self._focus_index = None
         self._edge_lookup = None
+        self._clusters = None              # semantic-cluster key table (graph/clusters.py)
 
     # ── construction from foreign graphs ────────────────────────────────
     @classmethod
@@ -89,7 +90,7 @@ class UnifiedGraph:
     # ── mutation (reference container.py:116-198) ───────────────────────
     def _invalidate(self) -> None:
         self._csr = None
-        self._rank_inputs = self._focus_index = self._edge_lookup = None
+        self._rank_inputs = self._focus_index = self._edge_lookup = self._clusters = None
         if self._dg is not None:
             self._dg.close()
             self._dg = None
@@ -101,7 +102,7 @@ class UnifiedGraph:
             self.nodes[node.id] = node
             self._invalidate()
             return
-        self._rank_inputs = None          # a merge can raise severity / risk, which the ranking reads
+        self._rank_inputs = self._clusters = None     # a merge can raise severity / risk and change attributes, which both read
         existing.last_seen = getattr(node, "last_seen", "") or _now_iso()
         existing.attributes.update(node.attributes)
         if SEVERITY_RANK.get(node.severity, 0) > SEVERITY_RANK.get(existing.severity, 0):

@@ -22,6 +22,7 @@ from __future__ import annotations
 import threading
 from typing import Any
 
+from .graph.clusters import semantic_clusters_view
 from .graph.container import UnifiedGraph
 from .graph.dependency_reach import ReachabilityReport, compute_dependency_reach
 from .graph.exposure import exposure_path_rows, materialize_attack_paths, ranked_attack_paths
@@ -190,6 +191,15 @@ class B200GraphStore:
         if g is None:
             g = UnifiedGraph(scan_id=scan_id, tenant_id=tenant_id)
         return fix_first_view(g, cve=cve, package=package, agent=agent, limit=limit)
+
+    def semantic_clusters_view(self, *, tenant_id: str = "", scan_id: str = "", kinds=None, min_members: int = 2, limit: int = 250) -> dict[str, Any]:
+        """The body of ``GET /v1/graph/clusters`` (reference api/routes/graph.py:1485-1528) for the resolved snapshot, rolled up on the
+        device; a missing snapshot gives the view of an empty graph, as the route's ``load_graph`` does.  The route keeps its own 503
+        when there is no snapshot at all, and turns the ``ValueError`` of an unknown kind into its 400."""
+        g = self._graph(tenant_id, scan_id)
+        if g is None:
+            g = UnifiedGraph(scan_id=scan_id, tenant_id=tenant_id)
+        return semantic_clusters_view(g, kinds=kinds, min_members=min_members, limit=limit)
 
     def ocsf_events(self, *, tenant_id: str = "", scan_id: str = "", product_version: str = "0.0.0", enrich_neighbors: bool = True, offset: int = 0,
                     limit: int | None = None) -> list[dict[str, Any]]:

@@ -485,6 +485,20 @@ const uint8_t *abb_union_result_w1(const abb_union_result *r);
 double abb_union_result_ms(const abb_union_result *r);            /* device time of the kernels, CUDA events */
 void abb_union_result_free(abb_union_result *r);
 
+/* ---- semantic clusters ---------------------------------------------------------------------------------------
+ * Replaces the roll-ups of build_semantic_clusters (agent_bom/graph/semantic_clusters.py:81-124).  The host interns each
+ * node's cluster keys into codes [n_nodes][2] (int32 in [0, k), -1 = none; ghosts have none) and passes per node a severity
+ * level (0 critical, 1 high, 2 medium, 3 low, 4 none), the rounded risk (f64, >= 0) and an entity-type index (< 64).
+ * abb_clusters_build_host builds the graph-constant tables (replacing earlier ones) and writes per cluster: member count,
+ * max risk, severity histogram [k][5], entity-type bit mask, and the number of distinct relationship codes its edges carry.
+ * An original edge counts once for each distinct cluster among its endpoints; relationship code 31 (a string outside the
+ * enum) is not counted here.  All pointers are host memory.
+ * abb_clusters_fetch_host copies, for the selected clusters in selection order, the member node indices in id-string order
+ * (count[c] each) and the (relationship code, edge count) pairs in code order (rel_nnz[c] each). */
+int abb_clusters_build_host(abb_graph *g, int64_t k, const int32_t *codes, const uint8_t *level, const double *risk, const uint8_t *etype,
+                            int64_t *count_out, double *max_risk_out, int64_t *hist_out, uint64_t *type_mask_out, int64_t *rel_nnz_out);
+int abb_clusters_fetch_host(abb_graph *g, int64_t n_sel, const int32_t *sel, int32_t *members_out, uint8_t *rel_out, int64_t *rel_count_out);
+
 #ifdef __cplusplus
 }
 #endif
