@@ -205,6 +205,11 @@ EXPORTS = {
     "abb_union_result_free": (None, [vp]),
     "abb_clusters_build_host": (C.c_int, [vp, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "abb_clusters_fetch_host": (C.c_int, [vp, i64, vp, vp, vp, vp]),
+    "abb_delta_table_host": (C.c_int, [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, i64, vp, vp, vp]),
+    "abb_delta_table_bytes": (i64, [vp]),
+    "abb_delta_build_host": (C.c_int, [vp, vp, vp, vp, vp, vp]),
+    "abb_delta_result_free": (None, [vp]),
+    "abb_delta_fetch_host": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
 }
 
 _lock = threading.Lock()

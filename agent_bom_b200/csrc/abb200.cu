@@ -31,6 +31,7 @@
 #include "nxcentral.cuh"
 #include "lateral.cuh"
 #include "clusters.cuh"
+#include "delta.cuh"
 #include "walk.cuh"
 #include "walkb.cuh"
 
@@ -288,6 +289,14 @@ struct abb_graph {
     DevBuf cl_members, cl_rel_key, cl_rel_cnt;
     std::vector<int64_t> cl_mem_off, cl_rel_off;
     int64_t cl_k = -1;
+    // snapshot-diff tables (delta_host.inl): id bytes + offsets of every node, sorted-order permutation; per real node the label
+    // bytes + offsets, status / severity codes and risk; per original edge a relationship slot, flags and (optionally) weight.
+    // dl_real = -1 until built.
+    DevBuf dl_ids, dl_ioff, dl_perm, dl_lbl, dl_loff, dl_stat, dl_sev, dl_risk, dl_erel, dl_eflag, dl_w;
+    int32_t dl_real = -1;
+    int64_t dl_ne = 0;
+    bool dl_has_w = false;
+    int64_t dl_union_limit = DL_UNION_LIMIT;
     // graph arrays of an uploaded graph (an adopted graph's belong to the caller)
     std::vector<DevBuf> owned_arrays;
 
@@ -474,6 +483,9 @@ extern "C" int abb_graph_set_option(abb_graph *g, const char *name, int64_t valu
     } else if (k == "nx_batch") {
         if (value < 0) return fail(ABB_ERR_ARG, "nx_batch must be >= 0");
         g->nx_batch = value;
+    } else if (k == "delta_union_limit") {
+        if (value < 0 || value > DL_UNION_LIMIT) return fail(ABB_ERR_ARG, "delta_union_limit must be in [0, 2^27]");
+        g->dl_union_limit = value;
     } else return fail(ABB_ERR_ARG, "unknown option '%s'", name);
     return ABB_OK;
 }
@@ -491,6 +503,7 @@ extern "C" int64_t abb_graph_get_option(const abb_graph *g, const char *name) {
     if (k == "last_host_chunks") return g->last_host_chunks;
     if (k == "big_limit") return g->big_limit;
     if (k == "nx_batch") return g->nx_batch;
+    if (k == "delta_union_limit") return g->dl_union_limit;
     return -1;
 }
 
@@ -1962,3 +1975,4 @@ extern "C" int abb_finding_context_host(abb_graph *g, int32_t max_depth, const i
 #include "nxcentral_host.inl"
 #include "lateral_host.inl"
 #include "clusters_host.inl"
+#include "delta_host.inl"

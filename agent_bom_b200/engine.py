@@ -575,6 +575,55 @@ class DeviceGraph:
             _lib.check(_lib.load().abb_clusters_fetch_host(h, sel.shape[0], sel.ctypes.data, members.ctypes.data, rel.ctypes.data, cnt.ctypes.data))
         return members, rel, cnt
 
+    def build_delta_table(self, n_real: int, ids: bytes, id_off, perm, labels: bytes, label_off, status, severity, risk, erel, eflag, weight=None) -> None:
+        """Store the graph's snapshot-diff tables (``abb_delta_table_host``), replacing earlier ones; freed with the graph."""
+        id_off, label_off = np.ascontiguousarray(id_off, np.int64), np.ascontiguousarray(label_off, np.int64)
+        perm = _i32(perm)
+        status, severity = np.ascontiguousarray(status, np.uint8), np.ascontiguousarray(severity, np.uint8)
+        risk = np.ascontiguousarray(risk, np.float64)
+        erel, eflag = np.ascontiguousarray(erel, np.uint8), np.ascontiguousarray(eflag, np.uint8)
+        if weight is not None:
+            weight = np.ascontiguousarray(weight, np.float64)
+        if id_off.shape != (self.n_nodes + 1,) or perm.shape != (self.n_nodes,) or label_off.shape != (n_real + 1,) or \
+                status.shape != (n_real,) or severity.shape != (n_real,) or risk.shape != (n_real,) or eflag.shape != erel.shape or \
+                (weight is not None and weight.shape != erel.shape):
+            raise ValueError("delta table inputs have the wrong shapes")
+        ids_buf = np.frombuffer(ids, np.uint8) if ids else np.zeros(1, np.uint8)
+        lbl_buf = np.frombuffer(labels, np.uint8) if labels else np.zeros(1, np.uint8)
+        with self._use() as h:
+            _lib.check(_lib.load().abb_delta_table_host(h, n_real, ids_buf.ctypes.data, id_off.ctypes.data, perm.ctypes.data, lbl_buf.ctypes.data,
+                                                        label_off.ctypes.data, status.ctypes.data, severity.ctypes.data, risk.ctypes.data, erel.shape[0],
+                                                        erel.ctypes.data, eflag.ctypes.data, None if weight is None else weight.ctypes.data))
+
+    def delta_table_bytes(self) -> int:
+        with self._use() as h:
+            return int(_lib.load().abb_delta_table_bytes(h))
+
+    def diff(self, old: "DeviceGraph", relmap_old, relmap_new) -> dict[str, np.ndarray]:
+        """Diff ``old`` -> this graph on the device (``abb_delta_build_host`` + ``abb_delta_fetch_host``); both need delta tables.
+        Returns ``nodes_added`` (this graph's indices) / ``nodes_removed`` (old's) in id order, ``changed_new`` / ``changed_old`` /
+        ``changed_flag`` node pairs in id order, ``edges_added`` / ``edges_removed`` edge indices and ``echanged_new`` /
+        ``echanged_old`` edge pairs in (source, target, relationship) order."""
+        rm_old = np.zeros(64, np.uint8)
+        rm_new = np.zeros(64, np.uint8)
+        rm_old[: len(relmap_old)] = relmap_old
+        rm_new[: len(relmap_new)] = relmap_new
+        sizes = np.zeros(6, np.int64)
+        lib = _lib.load()
+        res = _vp()
+        with self._use() as h, old._use() as ho:
+            _lib.check(lib.abb_delta_build_host(ho, h, rm_old.ctypes.data, rm_new.ctypes.data, C.byref(res), sizes.ctypes.data))
+        try:
+            na, nr, nc, ea, er, ec = (int(x) for x in sizes)
+            out = {"nodes_added": np.empty(na, np.int32), "nodes_removed": np.empty(nr, np.int32), "changed_new": np.empty(nc, np.int32),
+                   "changed_old": np.empty(nc, np.int32), "changed_flag": np.empty(nc, np.uint8), "edges_added": np.empty(ea, np.int32),
+                   "edges_removed": np.empty(er, np.int32), "echanged_new": np.empty(ec, np.int32), "echanged_old": np.empty(ec, np.int32)}
+            _lib.check(lib.abb_delta_fetch_host(res, *(out[k].ctypes.data for k in ("nodes_added", "nodes_removed", "changed_new", "changed_old", "changed_flag",
+                                                                                     "edges_added", "edges_removed", "echanged_new", "echanged_old"))))
+        finally:
+            lib.abb_delta_result_free(res)
+        return out
+
     def betweenness(self) -> np.ndarray:
         """``nx.betweenness_centrality`` of the graph as a DiGraph (``abb_betweenness_host``): f64 per node."""
         out = np.zeros(self.n_nodes, dtype=np.float64)

@@ -6,9 +6,11 @@
 Mirrors ``/root/reference/src/agent_bom/graph/__init__.py:8-100`` for the names the hot path needs.
 """
 
+from .alerts import compute_delta_alerts
 from .builder import build_unified_graph_from_report
 from .clusters import SEMANTIC_CLUSTER_KINDS, SemanticCluster, SemanticClusterExpansion, semantic_cluster_stats, semantic_clusters, semantic_clusters_view
 from .container import UnifiedGraph
+from .delta import snapshot_diff
 from .dependency_reach import PackageReachability, ReachabilityReport, VulnerabilityReachability, compute_dependency_reach
 from .envelope import EdgeIndex, exposure_path_for_attack_path, mcp_exposure_path_payload, serialize_attack_path, serialize_attack_paths
 from .fix_first import fix_first_view
@@ -24,4 +26,5 @@ __all__ = [
     "materialize_attack_paths", "node_risk_100", "ranked_attack_paths", "EdgeIndex", "exposure_path_for_attack_path", "mcp_exposure_path_payload",
     "serialize_attack_path", "serialize_attack_paths", "fix_first_view", "iter_ocsf_events", "ocsf_event",
     "SEMANTIC_CLUSTER_KINDS", "SemanticCluster", "SemanticClusterExpansion", "semantic_cluster_stats", "semantic_clusters", "semantic_clusters_view",
+    "snapshot_diff", "compute_delta_alerts",
 ]

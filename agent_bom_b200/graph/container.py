@@ -71,6 +71,7 @@ class UnifiedGraph:
         self._focus_index = None
         self._edge_lookup = None
         self._clusters = None              # semantic-cluster key table (graph/clusters.py)
+        self._delta = None                 # snapshot-diff tables (graph/delta.py)
 
     # ── construction from foreign graphs ────────────────────────────────
     @classmethod
@@ -90,7 +91,7 @@ class UnifiedGraph:
     # ── mutation (reference container.py:116-198) ───────────────────────
     def _invalidate(self) -> None:
         self._csr = None
-        self._rank_inputs = self._focus_index = self._edge_lookup = self._clusters = None
+        self._rank_inputs = self._focus_index = self._edge_lookup = self._clusters = self._delta = None
         if self._dg is not None:
             self._dg.close()
             self._dg = None
@@ -102,7 +103,7 @@ class UnifiedGraph:
             self.nodes[node.id] = node
             self._invalidate()
             return
-        self._rank_inputs = self._clusters = None     # a merge can raise severity / risk and change attributes, which both read
+        self._rank_inputs = self._clusters = self._delta = None     # a merge can raise severity / risk and change attributes, which they read
         existing.last_seen = getattr(node, "last_seen", "") or _now_iso()
         existing.attributes.update(node.attributes)
         if SEVERITY_RANK.get(node.severity, 0) > SEVERITY_RANK.get(existing.severity, 0):

@@ -214,6 +214,28 @@ class B200GraphStore:
         g = self._graph(tenant_id, scan_id)
         return None if g is None else compute_dependency_reach(g)
 
+    def diff_snapshots(self, scan_id_old: str, scan_id_new: str, *, tenant_id: str = "") -> dict[str, Any]:
+        """The body of ``GET /v1/graph/diff`` (reference db/graph_store.py:671-738), diffed on the device when the inner store is
+        SQLite-backed (``_db_path``, as for topology-first loading); otherwise the inner store's own ``diff_snapshots``.  A blank or
+        missing scan id is an empty snapshot: like the reference's ``scan_id = ?`` query, it never resolves to the latest one."""
+        from pathlib import Path
+
+        from .graph.delta import snapshot_diff
+
+        db_path = getattr(self._inner, "_db_path", None) if self._inner is not None else None
+        if db_path is None or not Path(db_path).exists():
+            inner = getattr(self._inner, "diff_snapshots", None) if self._inner is not None else None
+            if inner is None:
+                raise B200UnsupportedOperationError("B200GraphStore has no inner store to serve diff_snapshots()")
+            return inner(scan_id_old, scan_id_new, tenant_id=tenant_id)
+        tenant = normalize_tenant(tenant_id)
+
+        def snapshot(scan_id: str) -> UnifiedGraph:
+            g = self._graph(tenant, scan_id) if scan_id else None
+            return g if g is not None else UnifiedGraph(scan_id=scan_id, tenant_id=tenant, device=self._device)
+
+        return snapshot_diff(snapshot(scan_id_old), snapshot(scan_id_new), db_path=db_path, tenant_id=tenant)
+
     # ── everything else: the wrapped default store ──────────────────────
     def __getattr__(self, name: str):
         inner = self.__dict__.get("_inner")

@@ -499,6 +499,32 @@ int abb_clusters_build_host(abb_graph *g, int64_t k, const int32_t *codes, const
                             int64_t *count_out, double *max_risk_out, int64_t *hist_out, uint64_t *type_mask_out, int64_t *rel_nnz_out);
 int abb_clusters_fetch_host(abb_graph *g, int64_t n_sel, const int32_t *sel, int32_t *members_out, uint8_t *rel_out, int64_t *rel_count_out);
 
+/* ---- snapshot diff -------------------------------------------------------------------------------------------
+ * Replaces the set arithmetic of diff_snapshots (agent_bom/db/graph_store.py:671-738) and the direction / traversable / weight
+ * part of _edge_change_fingerprint (:764-773).  abb_delta_table_host stores a graph's diff tables (replacing earlier ones):
+ * the UTF-8 bytes of every node id (ghosts included) with offsets id_off[n_nodes + 1], perm[n_nodes] (sorted position -> node,
+ * the inverse of node_rank), per real node the label bytes with offsets label_off[n_real + 1], a status and a severity code
+ * (255: a string the host compares itself) and the risk (f64, compared with ==), and per original edge (graph.edges order) a
+ * relationship slot (< 64), flags (1 traversable, 2 bidirectional) and optionally the weight (NULL: not compared).
+ * abb_delta_build_host diffs two graphs with tables on one device.  relmap_* [64] map each graph's relationship slots to the
+ * rank of the relationship string among both graphs' strings.  It fails when the union of both id sets exceeds 2^27 ids (or
+ * the graphs' "delta_union_limit" option).  sizes_out[6] = {nodes added, nodes removed, node pairs changed, edges added, edges
+ * removed, edge pairs changed}; only real nodes count.  The answer stays on the device in *out, owned by the caller, so diffs
+ * may run concurrently on shared graphs.  abb_delta_fetch_host copies it: added nodes (new
+ * indices) and removed nodes (old indices) in id order; changed node pairs (new index, old index, flag: 1 changed, 2 equal
+ * unless a code-255 string or the OTHER entity type differs) in id order; added / removed edges (edge indices) and changed edge
+ * pairs (new edge, old edge) in (source, target, relationship) order.  All pointers are host memory. */
+int abb_delta_table_host(abb_graph *g, int32_t n_real, const uint8_t *ids, const int64_t *id_off, const int32_t *perm, const uint8_t *labels,
+                         const int64_t *label_off, const uint8_t *status, const uint8_t *severity, const double *risk, int64_t n_edges,
+                         const uint8_t *erel, const uint8_t *eflag, const double *weight);
+int64_t abb_delta_table_bytes(const abb_graph *g);               /* device bytes of the diff tables, 0 when none */
+typedef struct abb_delta_result abb_delta_result;
+int abb_delta_build_host(abb_graph *old_g, abb_graph *new_g, const uint8_t *relmap_old, const uint8_t *relmap_new, abb_delta_result **out,
+                         int64_t *sizes_out);
+void abb_delta_result_free(abb_delta_result *r);
+int abb_delta_fetch_host(const abb_delta_result *r, int32_t *nodes_added, int32_t *nodes_removed, int32_t *changed_new, int32_t *changed_old,
+                         uint8_t *changed_flag, int32_t *edges_added, int32_t *edges_removed, int32_t *echanged_new, int32_t *echanged_old);
+
 #ifdef __cplusplus
 }
 #endif
