@@ -156,9 +156,53 @@ struct DevBuf {
         cap = want;
         return ABB_OK;
     }
+    // exact size (`bytes` plus `spare`), filled with `bytes` of host memory on `st`
+    int upload(const void *src, size_t bytes, cudaStream_t st, size_t spare = 0) {
+        if (int rc = alloc(bytes + spare)) return rc;
+        if (bytes) CUDA_TRY(cudaMemcpyAsync(p, src, bytes, cudaMemcpyHostToDevice, st));
+        return ABB_OK;
+    }
     void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
     template <class T> T *as() const { return static_cast<T *>(p); }
 };
+
+// grows workspace buffer g->buf; needs `g` and `int rc` in scope and keeps the first error in rc
+#define ENS(buf, bytes) if (!rc) rc = g->buf.ensure(static_cast<size_t>(bytes))
+
+// One cub algorithm: `call(temp, bytes)` makes the cub call, once to size it and once to run it, so both share one argument list.
+// `tmp` grows to exactly what cub asks for; each caller names its own (calls on different streams run at the same time).
+template <class F>
+static int cub_run(DevBuf &tmp, F &&call) {
+    size_t bytes = 0;
+    CUDA_TRY(call(nullptr, bytes));
+    if (!tmp.p || bytes > tmp.cap) if (int rc = tmp.alloc(bytes)) return rc;
+    CUDA_TRY(call(tmp.p, bytes));
+    g_launches++;
+    return ABB_OK;
+}
+
+// exclusive prefix sum of n int64 values; `sync` waits for it
+static int scan_i64(DevBuf &tmp, const int64_t *in, int64_t *out, int64_t n, cudaStream_t st, bool sync = false) {
+    if (int rc = cub_run(tmp, [&](void *t, size_t &b) { return cub::DeviceScan::ExclusiveSum(t, b, in, out, static_cast<int>(n), st); })) return rc;
+    if (sync) CUDA_TRY(cudaStreamSynchronize(st));
+    return ABB_OK;
+}
+
+// positions k < n whose flag is set, in order, into pos; how many into *count (device memory)
+template <class Pos, class Flag, class Count, class N>
+static int select_flagged(DevBuf &tmp, Flag *flags, Pos *pos, Count *count, N n, cudaStream_t st) {
+    cub::CountingInputIterator<Pos> iota(0);
+    return cub_run(tmp, [&](void *t, size_t &b) { return cub::DeviceSelect::Flagged(t, b, iota, flags, pos, count, n, st); });
+}
+
+// blocks for `items` at `per_block` items each: at least one, and at most `per_sm` per SM when per_sm > 0
+static unsigned grid_for(int64_t items, int64_t per_block, int sm_count = 0, int per_sm = 0) {
+    int64_t b = (items + per_block - 1) / per_block;
+    if (per_sm > 0) b = std::min<int64_t>(b, static_cast<int64_t>(per_sm) * sm_count);
+    return static_cast<unsigned>(std::max<int64_t>(1, b));
+}
+
+static int ceil_log2_i64(int64_t n) { int b = 1; while ((1ll << b) < n) b++; return b; }
 
 // pinned host blocks, recycled across results (cudaHostAlloc is milliseconds)
 struct PinnedPool {
@@ -202,6 +246,18 @@ struct HostBlock {
     bool alloc(size_t n) { release(); p = g_pinned.get(n, &bytes); return p != nullptr; }
     void release() { g_pinned.put(p, bytes); p = nullptr; bytes = 0; }
     template <class T> T *as() const { return static_cast<T *>(p); }
+};
+
+// device-to-pinned-host copies on one stream: adds the bytes to *counted and keeps the first CUDA error
+struct Readback {
+    cudaStream_t st;
+    int64_t *counted;
+    cudaError_t err = cudaSuccess;
+    void keep(cudaError_t e) { if (err == cudaSuccess) err = e; }
+    void operator()(HostBlock &dst, const void *src, size_t bytes) {
+        *counted += static_cast<int64_t>(bytes);
+        if (err == cudaSuccess && bytes) err = cudaMemcpyAsync(dst.p, src, bytes, cudaMemcpyDeviceToHost, st);
+    }
 };
 
 // ------------------------------------------------------------------ graph handle
@@ -639,8 +695,6 @@ static int launch_block(const abb_graph *g, const WalkArgs &A, const BlockTier &
     return ABB_OK;
 }
 
-static int ceil_log2_i64(int64_t n) { int b = 1; while ((1ll << b) < n) b++; return b; }
-
 // Up to five tiers on one stream.  `A` carries spec/io and the first tier's work list (qlist/nq/nq_dev); every later
 // tier reads its work list and count from device memory, so nothing here waits for the GPU.
 //   S1  warp  + shared-memory bucketed hash/queue   (<= 256 queue entries)
@@ -747,14 +801,12 @@ static int enqueue_dedup_walk(abb_graph *g, const abb_walk_spec *spec, const abb
     const size_t q1 = static_cast<size_t>(nq) + 2;
     const uint32_t fl = spec->flags;
     int rc = ABB_OK;
-#define ENS(buf, bytes) if (!rc) rc = g->buf.ensure(bytes)
     ENS(dd_sig, q1 * 8); ENS(dd_ssig, q1 * 8); ENS(dd_q, q1 * 4); ENS(dd_sq, q1 * 4); ENS(dd_head, q1); ENS(dd_gid, q1 * 8); ENS(dd_hp, q1 * 8);
     ENS(dd_glen, q1 * 8); ENS(dd_goff, q1 * 8); ENS(dd_arena, q1 * 4 * L1_CAP); ENS(dd_memoff, q1 * 8); ENS(dd_memsrc, q1 * 4); ENS(dd_memstate, q1 * 4);
     ENS(dd_indiv, q1 * 4); ENS(dd_cnt, 8 * sizeof(unsigned long long));
     ENS(dd_lkey, q1 * 4); ENS(dd_lkey2, q1 * 4); ENS(dd_lgid, q1 * 4); ENS(dd_order, q1 * 4);
     ENS(dd_gstart, q1 * 8); ENS(dd_gcount, q1 * 4); ENS(dd_gmaxd, q1 * 4); ENS(dd_gflags, q1 * 4);
     if (fl & ABB_WALK_HIST) { ENS(dd_ghist, q1 * ABB_N_ENTITY_TYPES * 4); }
-#undef ENS
     if (rc) return rc;
     unsigned long long *cnt = g->dd_cnt.as<unsigned long long>();
     unsigned long long *sig = g->dd_sig.as<unsigned long long>(), *ssig = g->dd_ssig.as<unsigned long long>();
@@ -766,22 +818,15 @@ static int enqueue_dedup_walk(abb_graph *g, const abb_walk_spec *spec, const abb
     CUDA_TRY(cudaMemsetAsync(cnt, 0, 8 * sizeof(unsigned long long), st));
     CUDA_TRY(cudaMemsetAsync(glen, 0, q1 * 8, st));
     dedup_sig_kernel<<<blocks, 256, 0, st>>>(g->v, *spec, io->roots, nq, sig, qi); g_launches++;
-    // temp storage: the largest of the cub calls below
-    size_t t_sort = 0, t_scan = 0, t_sel = 0, t_scan2 = 0;
-    CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, t_sort, sig, ssig, qi, sq, static_cast<int>(nq), 0, SIG_BITS, st));
-    cub::TransformInputIterator<int64_t, HeadToI64, const uint8_t *> head64(head, HeadToI64());
-    CUDA_TRY(cub::DeviceScan::InclusiveSum(nullptr, t_scan, head64, gid, static_cast<int>(nq), st));
-    cub::CountingInputIterator<int64_t> iota(0);
-    CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, t_sel, iota, head, hp, cnt, static_cast<int>(nq), st));
-    CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, t_scan2, glen, goff, static_cast<int>(nq + 1), st));
-    size_t tmp = std::max(std::max(t_sort, t_scan), std::max(t_sel, t_scan2)) + 256;
-    if ((rc = g->dd_tmp.ensure(tmp))) return rc;
-    CUDA_TRY(cub::DeviceRadixSort::SortPairs(g->dd_tmp.p, t_sort, sig, ssig, qi, sq, static_cast<int>(nq), 0, SIG_BITS, st)); g_launches++;
+    if ((rc = cub_run(g->dd_tmp, [&](void *t, size_t &b) { return cub::DeviceRadixSort::SortPairs(t, b, sig, ssig, qi, sq, static_cast<int>(nq), 0, SIG_BITS, st); })))
+        return rc;
     dedup_heads_kernel<<<blocks, 256, 0, st>>>(ssig, sq, nq, head, indiv, cnt); g_launches++;
-    CUDA_TRY(cub::DeviceScan::InclusiveSum(g->dd_tmp.p, t_scan, head64, gid, static_cast<int>(nq), st)); g_launches++;
-    CUDA_TRY(cub::DeviceSelect::Flagged(g->dd_tmp.p, t_sel, iota, head, hp, cnt, static_cast<int>(nq), st)); g_launches++;
+    cub::TransformInputIterator<int64_t, HeadToI64, const uint8_t *> head64(head, HeadToI64());
+    if ((rc = cub_run(g->dd_tmp, [&](void *t, size_t &b) { return cub::DeviceScan::InclusiveSum(t, b, head64, gid, static_cast<int>(nq), st); }))) return rc;
+    if ((rc = select_flagged(g->dd_tmp, head, hp, cnt, static_cast<int>(nq), st))) return rc;
     dedup_groups_kernel<<<static_cast<unsigned>((nq + 1 + 255) / 256), 256, 0, st>>>(g->v, *spec, io->roots, sq, hp, cnt, glen, memoff); g_launches++;
-    CUDA_TRY(cub::DeviceScan::ExclusiveSum(g->dd_tmp.p, t_scan2, glen, goff, static_cast<int>(nq + 1), st)); g_launches++;
+    // glen is passed non-const here, unlike scan_i64's input: a different cub instantiation
+    if ((rc = cub_run(g->dd_tmp, [&](void *t, size_t &b) { return cub::DeviceScan::ExclusiveSum(t, b, glen, goff, static_cast<int>(nq + 1), st); }))) return rc;
     dedup_roots_kernel<<<blocks, 256, 0, st>>>(g->v, *spec, io->roots, sq, hp, cnt, goff, g->dd_arena.as<int32_t>()); g_launches++;
     dedup_members_kernel<<<blocks, 256, 0, st>>>(g->v, *spec, io->roots, sq, head, gid, goff, g->dd_arena.as<int32_t>(), g->dd_memsrc.as<int32_t>(),
                                                   g->dd_memstate.as<int32_t>(), indiv, cnt); g_launches++;
@@ -801,16 +846,14 @@ static int enqueue_dedup_walk(abb_graph *g, const abb_walk_spec *spec, const abb
         uint32_t *lkey = g->dd_lkey.as<uint32_t>(), *lkey2 = g->dd_lkey2.as<uint32_t>();
         int32_t *lgid = g->dd_lgid.as<int32_t>(), *order = g->dd_order.as<int32_t>();
         dedup_locality_keys_kernel<<<blocks, 256, 0, st>>>(cnt, goff, g->dd_arena.as<int32_t>(), lkey, lgid, nq); g_launches++;
-        size_t t_ls = 0;
-        CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, t_ls, lkey, lkey2, lgid, order, static_cast<int>(nq), 0, 32, st));
-        if ((rc = g->dd_tmp.ensure(std::max(tmp, t_ls + 256)))) return rc;
-        CUDA_TRY(cub::DeviceRadixSort::SortPairs(g->dd_tmp.p, t_ls, lkey, lkey2, lgid, order, static_cast<int>(nq), 0, 32, st)); g_launches++;
+        if ((rc = cub_run(g->dd_tmp, [&](void *t, size_t &b) { return cub::DeviceRadixSort::SortPairs(t, b, lkey, lkey2, lgid, order, static_cast<int>(nq), 0, 32, st); })))
+            return rc;
         C.qlist = order;
     }
     C.depth_bias = 1; C.hist_roots = 1;
     C.mem_off = memoff; C.mem_src = g->dd_memsrc.as<int32_t>(); C.mem_state = g->dd_memstate.as<int32_t>();
     if ((rc = enqueue_tiers(g, C, nq, ctl, st))) return rc;
-    dedup_share_kernel<<<static_cast<unsigned>(std::min<int64_t>((nq + 255) / 256, static_cast<int64_t>(g->sm_count) * 8)), 256, 0, st>>>(
+    dedup_share_kernel<<<grid_for(nq, 256, g->sm_count, 8), 256, 0, st>>>(
         sq, gid, g->dd_memstate.as<int32_t>(), cnt, C.io.q_start, C.io.q_count, C.io.q_maxd, C.io.q_flags, C.io.q_hist, io->q_start, io->q_count, io->q_maxd,
         io->q_flags, (fl & ABB_WALK_HIST) ? io->q_hist : nullptr, indiv, cnt);
     g_launches++;
@@ -986,6 +1029,47 @@ extern "C" const uint32_t *abb_walk_result_edges(const abb_walk_result *r) { ret
 extern "C" int64_t abb_walk_result_h2d_bytes(const abb_walk_result *r) { return r->h2d; }
 extern "C" int64_t abb_walk_result_d2h_bytes(const abb_walk_result *r) { return r->d2h; }
 
+// ------------------------------------------------------------------ steps shared by the host walks
+// fails when a walk of either set (canonical, individual) outgrew the last storage tier; the walk's stream must be idle
+static int check_tier_fatal(abb_graph *g) {
+    unsigned long long fatal = 0, fatal2 = 0;
+    CUDA_TRY(cudaMemcpy(&fatal, g->ctl.as<unsigned long long>() + CTL_FATAL, sizeof fatal, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(&fatal2, g->ctl.as<unsigned long long>() + CTL_SET + CTL_FATAL, sizeof fatal2, cudaMemcpyDeviceToHost));
+    if (fatal || fatal2) return fail(ABB_ERR_CAPACITY, "a traversal outgrew the global scratch tier (more than n_nodes+4096 queue entries)");
+    return ABB_OK;
+}
+
+// the non-zero histogram columns and the largest count of nq rows, into g->hist_info once st has been synchronised
+static int scan_hist_columns(abb_graph *g, const uint32_t *q_hist, int64_t nq, cudaStream_t st) {
+    if (int rc = g->d_histinfo.ensure(2 * sizeof(unsigned long long))) return rc;
+    CUDA_TRY(cudaMemsetAsync(g->d_histinfo.p, 0, 2 * sizeof(unsigned long long), st));
+    hist_columns_kernel<<<static_cast<unsigned>(g->sm_count) * 8, 256, 0, st>>>(q_hist, nq * ABB_N_ENTITY_TYPES, g->d_histinfo.as<unsigned long long>());
+    g_launches++;
+    CUDA_TRY(cudaMemcpyAsync(g->hist_info, g->d_histinfo.p, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    return ABB_OK;
+}
+
+// r's packed-histogram layout from g->hist_info: the non-zero columns, at 2 bytes per count when every count fits
+static HistCols hist_layout(const abb_graph *g, abb_walk_result *r) {
+    HistCols hc{};
+    r->hist_is_packed = true;
+    r->hist_mask = static_cast<uint32_t>(g->hist_info[0]);
+    for (int t = 0; t < ABB_N_ENTITY_TYPES; t++) if (r->hist_mask >> t & 1u) hc.col[hc.k++] = static_cast<uint8_t>(t);
+    r->hist_k = hc.k;
+    r->hist_width = g->hist_info[1] < 65536ull ? 2 : 4;
+    return hc;
+}
+
+// size hints for the next host walk: the largest node arena so far and the last batch; for a plain walk (one root per query, no
+// parents / depths / edges / targets) also what the chunked path sizes its pieces from
+static void note_walk_size(abb_graph *g, const abb_walk_spec *spec, int64_t nq, int64_t nodes, bool plain) {
+    g->hint_nodes = std::max(g->hint_nodes, nodes);
+    g->hint_nq = nq; g->hint_last_nodes = nodes;
+    if (!plain) return;
+    if (g->plain_nq != nq || memcmp(&g->plain_spec, spec, sizeof *spec) != 0) g->chunk_hint_nq = -1;
+    g->plain_spec = *spec; g->plain_nq = nq; g->plain_nodes = nodes;
+}
+
 // stage inputs, run (re-run once if the arenas were too small), leave results on the device
 // `direct_nodes`: when the result size is known from the previous call, the walk kernels write the node arena
 // straight into that pinned host block (UVA), so the PCIe transfer of the largest output overlaps the traversal
@@ -1000,16 +1084,15 @@ static int walk_device_stage(abb_graph *g, const abb_walk_spec *spec, const int3
     const int64_t n_roots = root_off ? root_off[nq] : nq;
     if (n_roots < 0) return fail(ABB_ERR_ARG, "bad root_off");
     const size_t q1 = static_cast<size_t>(nq) + 1;
-    if (int rc = g->d_roots.ensure(static_cast<size_t>(n_roots + 1) * 4)) return rc;
-    if (root_off) if (int rc = g->d_root_off.ensure(q1 * 8)) return rc;
-    if (fl & ABB_WALK_TARGET) if (int rc = g->d_targets.ensure(q1 * 4)) return rc;
-    if (int rc = g->d_qstart.ensure(q1 * 8)) return rc;
-    if (int rc = g->d_qcount.ensure(q1 * 4)) return rc;
-    if (int rc = g->d_qmaxd.ensure(q1 * 4)) return rc;
-    if (int rc = g->d_qflags.ensure(q1 * 4)) return rc;
-    if (fl & ABB_WALK_EDGES) { if (int rc = g->d_qestart.ensure(q1 * 8)) return rc; if (int rc = g->d_qecount.ensure(q1 * 8)) return rc; }
-    if (fl & ABB_WALK_HIST) if (int rc = g->d_qhist.ensure(q1 * ABB_N_ENTITY_TYPES * 4)) return rc;
-    if (int rc = g->d_totals.ensure(3 * sizeof(unsigned long long))) return rc;
+    int rc = ABB_OK;
+    ENS(d_roots, (n_roots + 1) * 4);
+    if (root_off) ENS(d_root_off, q1 * 8);
+    if (fl & ABB_WALK_TARGET) ENS(d_targets, q1 * 4);
+    ENS(d_qstart, q1 * 8); ENS(d_qcount, q1 * 4); ENS(d_qmaxd, q1 * 4); ENS(d_qflags, q1 * 4);
+    if (fl & ABB_WALK_EDGES) { ENS(d_qestart, q1 * 8); ENS(d_qecount, q1 * 8); }
+    if (fl & ABB_WALK_HIST) ENS(d_qhist, q1 * ABB_N_ENTITY_TYPES * 4);
+    ENS(d_totals, 3 * sizeof(unsigned long long));
+    if (rc) return rc;
     *h2d = 0;
     if (n_roots && !roots_staged) { CUDA_TRY(cudaMemcpyAsync(g->d_roots.p, roots, static_cast<size_t>(n_roots) * 4, cudaMemcpyHostToDevice, st)); *h2d += n_roots * 4; }
     if (root_off) { CUDA_TRY(cudaMemcpyAsync(g->d_root_off.p, root_off, q1 * 8, cudaMemcpyHostToDevice, st)); *h2d += static_cast<int64_t>(q1) * 8; }
@@ -1028,10 +1111,11 @@ static int walk_device_stage(abb_graph *g, const abb_walk_spec *spec, const int3
         direct = direct_nodes->alloc(static_cast<size_t>(node_cap) * 4);
     }
     for (int attempt = 0; attempt < 3; attempt++) {
-        if (!direct) if (int rc = g->d_nodes.ensure(static_cast<size_t>(node_cap) * 4)) return rc;
-        if (fl & ABB_WALK_PARENTS) if (int rc = g->d_parent.ensure(static_cast<size_t>(node_cap) * 4)) return rc;
-        if (fl & ABB_WALK_DEPTHS) if (int rc = g->d_depth.ensure(static_cast<size_t>(node_cap) * 4)) return rc;
-        if (fl & ABB_WALK_EDGES) if (int rc = g->d_edges.ensure(static_cast<size_t>(edge_cap) * 4)) return rc;
+        if (!direct) ENS(d_nodes, node_cap * 4);
+        if (fl & ABB_WALK_PARENTS) ENS(d_parent, node_cap * 4);
+        if (fl & ABB_WALK_DEPTHS) ENS(d_depth, node_cap * 4);
+        if (fl & ABB_WALK_EDGES) ENS(d_edges, edge_cap * 4);
+        if (rc) return rc;
         abb_walk_io io{};
         io.n_queries = nq; io.roots = g->d_roots.as<int32_t>(); io.root_off = root_off ? g->d_root_off.as<int64_t>() : nullptr;
         io.targets = (fl & ABB_WALK_TARGET) ? g->d_targets.as<int32_t>() : nullptr;
@@ -1049,32 +1133,17 @@ static int walk_device_stage(abb_graph *g, const abb_walk_spec *spec, const int3
         CUDA_TRY(cudaEventRecord(g->ev[1], st));
         g->walk_timed = true;
         const bool scan_hist = (fl & ABB_WALK_HIST) && g->hist_pack && nq >= 1024;
-        if (scan_hist) {
-            if (int rc = g->d_histinfo.ensure(2 * sizeof(unsigned long long))) return rc;
-            CUDA_TRY(cudaMemsetAsync(g->d_histinfo.p, 0, 2 * sizeof(unsigned long long), st));
-            hist_columns_kernel<<<static_cast<unsigned>(g->sm_count) * 8, 256, 0, st>>>(io.q_hist, nq * ABB_N_ENTITY_TYPES, g->d_histinfo.as<unsigned long long>());
-            g_launches++;
-            CUDA_TRY(cudaMemcpyAsync(g->hist_info, g->d_histinfo.p, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-        }
+        if (scan_hist) if ((rc = scan_hist_columns(g, io.q_hist, nq, st))) return rc;
         CUDA_TRY(cudaMemcpyAsync(totals, g->d_totals.p, 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaStreamSynchronize(st));
         g->hist_info_valid = scan_hist;
-        unsigned long long fatal = 0, fatal2 = 0;
-        CUDA_TRY(cudaMemcpy(&fatal, g->ctl.as<unsigned long long>() + CTL_FATAL, sizeof fatal, cudaMemcpyDeviceToHost));
-        CUDA_TRY(cudaMemcpy(&fatal2, g->ctl.as<unsigned long long>() + CTL_SET + CTL_FATAL, sizeof fatal2, cudaMemcpyDeviceToHost));
-        if (fatal || fatal2) return fail(ABB_ERR_CAPACITY, "a traversal outgrew the global scratch tier (more than n_nodes+4096 queue entries)");
+        if ((rc = check_tier_fatal(g))) return rc;
         *io_out = io;
         const bool fits = static_cast<int64_t>(totals[0]) <= node_cap && (!(fl & ABB_WALK_EDGES) || static_cast<int64_t>(totals[1]) <= edge_cap);
-        g->hint_nodes = std::max<int64_t>(g->hint_nodes, static_cast<int64_t>(totals[0]));
-        g->hint_nq = nq; g->hint_last_nodes = static_cast<int64_t>(totals[0]);
+        const bool plain = !root_off && !(fl & (ABB_WALK_PARENTS | ABB_WALK_DEPTHS | ABB_WALK_EDGES | ABB_WALK_TARGET));
+        note_walk_size(g, spec, nq, static_cast<int64_t>(totals[0]), fits && plain);
         g->hint_edges = std::max<int64_t>(g->hint_edges, static_cast<int64_t>(totals[1]));
-        if (fits) {
-            if (!root_off && !(fl & (ABB_WALK_PARENTS | ABB_WALK_DEPTHS | ABB_WALK_EDGES | ABB_WALK_TARGET))) {
-                if (g->plain_nq != nq || memcmp(&g->plain_spec, spec, sizeof *spec) != 0) g->chunk_hint_nq = -1;
-                g->plain_spec = *spec; g->plain_nq = nq; g->plain_nodes = static_cast<int64_t>(totals[0]);
-            }
-            return ABB_OK;
-        }
+        if (fits) return ABB_OK;
         if (direct) { direct_nodes->release(); direct = false; }     // estimate too small: fall back to a device arena
         node_cap = std::max<int64_t>(node_cap, static_cast<int64_t>(totals[0]));
         edge_cap = std::max<int64_t>(edge_cap, static_cast<int64_t>(totals[1]));
@@ -1106,28 +1175,17 @@ static int walk_collect(abb_graph *g, const abb_walk_spec *spec, const abb_walk_
     if (fl & ABB_WALK_EDGES) ok = ok && r->q_estart.alloc(q * 8) && r->q_ecount.alloc(q * 8) && r->edges.alloc(te * 4);
     const bool pack = (fl & ABB_WALK_HIST) && g->hist_info_valid;
     g->hist_info_valid = false;
-    HistCols hc{};
-    if (pack) {
-        r->hist_is_packed = true;
-        r->hist_mask = static_cast<uint32_t>(g->hist_info[0]);
-        for (int t = 0; t < ABB_N_ENTITY_TYPES; t++) if (r->hist_mask >> t & 1u) hc.col[hc.k++] = static_cast<uint8_t>(t);
-        r->hist_k = hc.k;
-        r->hist_width = g->hist_info[1] < 65536ull ? 2 : 4;
-        ok = ok && (hc.k == 0 || r->q_hist_packed.alloc(q * hc.k * r->hist_width));
-    } else if (fl & ABB_WALK_HIST) ok = ok && r->q_hist.alloc(q * ABB_N_ENTITY_TYPES * 4);
+    const HistCols hc = pack ? hist_layout(g, r.get()) : HistCols{};
+    if (pack) ok = ok && (hc.k == 0 || r->q_hist_packed.alloc(q * hc.k * r->hist_width));
+    else if (fl & ABB_WALK_HIST) ok = ok && r->q_hist.alloc(q * ABB_N_ENTITY_TYPES * 4);
     if (fl & ABB_WALK_PARENTS) ok = ok && r->parent.alloc(tn * 4);
     if (fl & ABB_WALK_DEPTHS) ok = ok && r->depth.alloc(tn * 4);
     if (!ok) return fail(ABB_ERR_NOMEM, "pinned host allocation failed");
-    auto d2h = [&](HostBlock &dst, const void *src, size_t bytes) -> cudaError_t {
-        r->d2h += static_cast<int64_t>(bytes);
-        return bytes ? cudaMemcpyAsync(dst.p, src, bytes, cudaMemcpyDeviceToHost, st) : cudaSuccess;
-    };
-    cudaError_t e = cudaSuccess;
-    auto acc = [&](cudaError_t x) { if (e == cudaSuccess) e = x; };
-    if (with_slices) acc(d2h(r->q_start, io.q_start, q * 8));
-    acc(d2h(r->q_count, io.q_count, q * 4)); acc(d2h(r->q_maxd, io.q_maxd, q * 4)); acc(d2h(r->q_flags, io.q_flags, q * 4));
-    if (have_nodes) r->d2h += static_cast<int64_t>((totals[2] ? totals[2] : static_cast<unsigned long long>(tn)) * 4); else if (with_slices) acc(d2h(r->nodes, io.nodes, tn * 4));
-    if (fl & ABB_WALK_EDGES) { acc(d2h(r->q_estart, io.q_estart, q * 8)); acc(d2h(r->q_ecount, io.q_ecount, q * 8)); acc(d2h(r->edges, io.edges, te * 4)); }
+    Readback d2h{st, &r->d2h};
+    if (with_slices) d2h(r->q_start, io.q_start, q * 8);
+    d2h(r->q_count, io.q_count, q * 4); d2h(r->q_maxd, io.q_maxd, q * 4); d2h(r->q_flags, io.q_flags, q * 4);
+    if (have_nodes) r->d2h += static_cast<int64_t>((totals[2] ? totals[2] : static_cast<unsigned long long>(tn)) * 4); else if (with_slices) d2h(r->nodes, io.nodes, tn * 4);
+    if (fl & ABB_WALK_EDGES) { d2h(r->q_estart, io.q_estart, q * 8); d2h(r->q_ecount, io.q_ecount, q * 8); d2h(r->edges, io.edges, te * 4); }
     if (pack) {
         if (hc.k) {
             const size_t pbytes = q * hc.k * r->hist_width;
@@ -1136,14 +1194,14 @@ static int walk_collect(abb_graph *g, const abb_walk_spec *spec, const abb_walk_
             if (r->hist_width == 2) hist_pack_kernel<uint16_t><<<grid, 256, 0, st>>>(io.q_hist, nq, hc, g->d_hist_packed.as<uint16_t>());
             else hist_pack_kernel<uint32_t><<<grid, 256, 0, st>>>(io.q_hist, nq, hc, g->d_hist_packed.as<uint32_t>());
             g_launches++;
-            acc(cudaGetLastError());
-            acc(d2h(r->q_hist_packed, g->d_hist_packed.p, pbytes));
+            d2h.keep(cudaGetLastError());
+            d2h(r->q_hist_packed, g->d_hist_packed.p, pbytes);
         }
-    } else if (fl & ABB_WALK_HIST) acc(d2h(r->q_hist, io.q_hist, q * ABB_N_ENTITY_TYPES * 4));
-    if (fl & ABB_WALK_PARENTS) acc(d2h(r->parent, io.parent, tn * 4));
-    if (fl & ABB_WALK_DEPTHS) acc(d2h(r->depth, io.depth, tn * 4));
-    if (e == cudaSuccess && sync) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) return fail(ABB_ERR_CUDA, "D2H failed: %s", cudaGetErrorString(e));
+    } else if (fl & ABB_WALK_HIST) d2h(r->q_hist, io.q_hist, q * ABB_N_ENTITY_TYPES * 4);
+    if (fl & ABB_WALK_PARENTS) d2h(r->parent, io.parent, tn * 4);
+    if (fl & ABB_WALK_DEPTHS) d2h(r->depth, io.depth, tn * 4);
+    if (sync && d2h.err == cudaSuccess) d2h.err = cudaStreamSynchronize(st);
+    if (d2h.err != cudaSuccess) return fail(ABB_ERR_CUDA, "D2H failed: %s", cudaGetErrorString(d2h.err));
     *out = r.release();
     return ABB_OK;
 }
@@ -1177,7 +1235,6 @@ static int walk_host_chunked(abb_graph *g, const abb_walk_spec *spec, const int3
     const size_t q = static_cast<size_t>(nq), q1 = q + 1;
     const bool hist = (fl & ABB_WALK_HIST) != 0;
     int rc = ABB_OK;
-#define ENS(buf, bytes) if (!rc) rc = g->buf.ensure(static_cast<size_t>(bytes))
     ENS(d_roots, q1 * 4); ENS(d_qstart, q1 * 8); ENS(d_qcount, q1 * 4); ENS(d_qmaxd, q1 * 4); ENS(d_qflags, q1 * 4);
     if (hist) ENS(d_qhist, q1 * ABB_N_ENTITY_TYPES * 4);
     ENS(d_totals, 3 * sizeof(unsigned long long));
@@ -1206,13 +1263,10 @@ static int walk_host_chunked(abb_graph *g, const abb_walk_spec *spec, const int3
     }
     CUDA_TRY(cudaMemsetAsync(g->ck_counts.p, 0, 64 * 8, st));
     chunk_key_kernel<<<qblocks, 256, 0, st>>>(sig, nq, K, g->ck_key.as<uint32_t>(), g->ck_idx.as<int32_t>(), g->ck_counts.as<unsigned long long>()); g_launches++;
-    {
-        size_t tmp = 0;
-        CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tmp, g->ck_key.as<uint32_t>(), g->ck_key2.as<uint32_t>(), g->ck_idx.as<int32_t>(), g->ck_order.as<int32_t>(), static_cast<int>(nq), 0, 6, st));
-        if ((rc = g->ck_tmp.ensure(tmp + 16))) { drain(); return rc; }
-        CUDA_TRY(cub::DeviceRadixSort::SortPairs(g->ck_tmp.p, tmp, g->ck_key.as<uint32_t>(), g->ck_key2.as<uint32_t>(), g->ck_idx.as<int32_t>(), g->ck_order.as<int32_t>(), static_cast<int>(nq), 0, 6, st));
-        g_launches++;
-    }
+    if ((rc = cub_run(g->ck_tmp, [&](void *t, size_t &b) {
+             return cub::DeviceRadixSort::SortPairs(t, b, g->ck_key.as<uint32_t>(), g->ck_key2.as<uint32_t>(), g->ck_idx.as<int32_t>(), g->ck_order.as<int32_t>(),
+                                                    static_cast<int>(nq), 0, 6, st);
+         }))) { drain(); return rc; }
     const int32_t *order = g->ck_order.as<int32_t>();      // order[i] = caller index of the i-th query in chunk order
     gather_i32_kernel<<<qblocks, 256, 0, st>>>(g->d_roots.as<int32_t>(), order, g->ck_roots.as<int32_t>(), nq); g_launches++;
     unsigned long long counts[64] = {0};
@@ -1245,10 +1299,7 @@ static int walk_host_chunked(abb_graph *g, const abb_walk_spec *spec, const int3
             if (int erc = enqueue_walk(g, spec, &io, st)) { drain(); return erc; }
             CUDA_TRY(cudaMemcpyAsync(totals, g->d_totals.p, 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
             CUDA_TRY(cudaStreamSynchronize(st));
-            unsigned long long fatal = 0, fatal2 = 0;
-            CUDA_TRY(cudaMemcpy(&fatal, g->ctl.as<unsigned long long>() + CTL_FATAL, sizeof fatal, cudaMemcpyDeviceToHost));
-            CUDA_TRY(cudaMemcpy(&fatal2, g->ctl.as<unsigned long long>() + CTL_SET + CTL_FATAL, sizeof fatal2, cudaMemcpyDeviceToHost));
-            if (fatal || fatal2) { drain(); return fail(ABB_ERR_CAPACITY, "a traversal outgrew the global scratch tier (more than n_nodes+4096 queue entries)"); }
+            if ((rc = check_tier_fatal(g))) { drain(); return rc; }
             if (static_cast<int64_t>(totals[0]) <= cap) done = true; else cap = static_cast<int64_t>(totals[0]) + 4096;
         }
         if (!done) { drain(); return fail(ABB_ERR_CAPACITY, "walk arenas still too small after resize"); }
@@ -1282,26 +1333,13 @@ static int walk_host_chunked(abb_graph *g, const abb_walk_spec *spec, const int3
     g_launches += 4;
     const bool scan_hist = hist && g->hist_pack && nq >= 1024;
     if (scan_hist) {
-        if ((rc = g->d_histinfo.ensure(2 * sizeof(unsigned long long)))) { drain(); return rc; }
-        CUDA_TRY(cudaMemsetAsync(g->d_histinfo.p, 0, 2 * sizeof(unsigned long long), st));
-        hist_columns_kernel<<<sgrid, 256, 0, st>>>(g->d_qhist.as<uint32_t>(), nq * ABB_N_ENTITY_TYPES, g->d_histinfo.as<unsigned long long>());
-        g_launches++;
-        CUDA_TRY(cudaMemcpyAsync(g->hist_info, g->d_histinfo.p, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+        if ((rc = scan_hist_columns(g, g->d_qhist.as<uint32_t>(), nq, st))) { drain(); return rc; }
         CUDA_TRY(cudaStreamSynchronize(st));
     }
-    cudaError_t e = cudaGetLastError();
-    auto d2h = [&](HostBlock &dst, const void *src, size_t bytes) {
-        r->d2h += static_cast<int64_t>(bytes);
-        if (e == cudaSuccess && bytes) e = cudaMemcpyAsync(dst.p, src, bytes, cudaMemcpyDeviceToHost, st);
-    };
+    Readback d2h{st, &r->d2h, cudaGetLastError()};
     d2h(r->q_start, g->ck_qstart.p, q * 8); d2h(r->q_count, g->ck_qcount.p, q * 4); d2h(r->q_maxd, g->ck_qmaxd.p, q * 4); d2h(r->q_flags, g->ck_qflags.p, q * 4);
     if (scan_hist) {
-        HistCols hc{};
-        r->hist_is_packed = true;
-        r->hist_mask = static_cast<uint32_t>(g->hist_info[0]);
-        for (int t = 0; t < ABB_N_ENTITY_TYPES; t++) if (r->hist_mask >> t & 1u) hc.col[hc.k++] = static_cast<uint8_t>(t);
-        r->hist_k = hc.k;
-        r->hist_width = g->hist_info[1] < 65536ull ? 2 : 4;
+        const HistCols hc = hist_layout(g, r.get());
         if (hc.k) {
             const size_t pbytes = q * hc.k * r->hist_width;
             if (!r->q_hist_packed.alloc(pbytes)) { drain(); return fail(ABB_ERR_NOMEM, "pinned host allocation failed"); }
@@ -1318,16 +1356,14 @@ static int walk_host_chunked(abb_graph *g, const abb_walk_spec *spec, const int3
         g_launches++;
         d2h(r->q_hist, g->ck_qhist.p, q * ABB_N_ENTITY_TYPES * 4);
     }
-#undef ENS
+    cudaError_t &e = d2h.err;
     if (e == cudaSuccess) e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(cst);
     if (e != cudaSuccess) { drain(); return fail(ABB_ERR_CUDA, "chunked walk failed: %s", cudaGetErrorString(e)); }
     g->hist_info_valid = false;
+    note_walk_size(g, spec, nq, node_base, true);
     g->chunk_hint = produced; g->chunk_hint_nq = nq;
-    g->hint_nodes = std::max<int64_t>(g->hint_nodes, node_base);
-    g->hint_nq = nq; g->hint_last_nodes = node_base;
-    g->plain_spec = *spec; g->plain_nq = nq; g->plain_nodes = node_base;
     g->last_host_chunks = K;
     *out = r.release();
     return ABB_OK;
@@ -1352,22 +1388,12 @@ extern "C" int abb_walk_host(abb_graph *g, const abb_walk_spec *spec, const int3
 }
 
 // ------------------------------------------------------------------ exposure-path rows
-static int scan_i64(abb_graph *g, const int64_t *in, int64_t *out, int64_t n, cudaStream_t st) {
-    size_t tmp = 0;
-    CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tmp, in, out, static_cast<int>(n), st));
-    if (int rc = g->p_scan_tmp.ensure(tmp + 16)) return rc;
-    CUDA_TRY(cub::DeviceScan::ExclusiveSum(g->p_scan_tmp.p, tmp, in, out, static_cast<int>(n), st));
-    g_launches++;
-    return ABB_OK;
-}
-
 static int ensure_server_table(abb_graph *g, cudaStream_t st) {
     if (g->srv_table_ready) return ABB_OK;
     const size_t n = static_cast<size_t>(g->v.n) + 1;
     if (int rc = g->srv_cred.ensure(n * 4)) return rc;
     if (int rc = g->srv_tool.ensure(n * 4)) return rc;
-    const int64_t blocks = std::min<int64_t>((g->v.n + 255) / 256, static_cast<int64_t>(g->sm_count) * 16);
-    const unsigned grid = static_cast<unsigned>(std::max<int64_t>(1, blocks));
+    const unsigned grid = grid_for(g->v.n, 256, g->sm_count, 16);
     server_table_kernel<<<grid, 256, 0, st>>>(g->v, g->srv_cred.as<int32_t>(), g->srv_tool.as<int32_t>());
     g_launches++;
     // principal rows of every server (paths.cuh server_rows_kernel): count, scan in place, fill
@@ -1376,7 +1402,7 @@ static int ensure_server_table(abb_graph *g, cudaStream_t st) {
     CUDA_TRY(cudaMemsetAsync(roff, 0, n * 8, st));
     server_rows_kernel<false><<<grid, 256, 0, st>>>(g->v, g->srv_cred.as<int32_t>(), g->srv_tool.as<int32_t>(), roff, nullptr, nullptr);
     g_launches++;
-    if (int rc = scan_i64(g, roff, roff, static_cast<int64_t>(n), st)) return rc;
+    if (int rc = scan_i64(g->p_scan_tmp, roff, roff, static_cast<int64_t>(n), st)) return rc;
     int64_t total = 0;
     CUDA_TRY(cudaMemcpyAsync(&total, roff + g->v.n, 8, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
@@ -1440,9 +1466,9 @@ static int ensure_exposure_tables(abb_graph *g, cudaStream_t st) {
     CUDA_TRY(cudaMemsetAsync(A.x_overflow, 0, 4, st));
     const unsigned grid = warp_grid(g, (n + 31) / 32);
     node_links_kernel<false><<<grid, 256, 0, st>>>(A); g_launches++;
-    if ((rc = scan_i64(g, A.x_loff, A.x_loff, n + 1, st))) return rc;
+    if ((rc = scan_i64(g->p_scan_tmp, A.x_loff, A.x_loff, n + 1, st))) return rc;
     template_kernel<false><<<grid, 256, 0, st>>>(A); g_launches++;
-    if ((rc = scan_i64(g, A.x_toff, A.x_toff, n + 1, st))) return rc;
+    if ((rc = scan_i64(g->p_scan_tmp, A.x_toff, A.x_toff, n + 1, st))) return rc;
     int64_t NL = 0, TR = 0;
     CUDA_TRY(cudaMemcpyAsync(&NL, A.x_loff + n, 8, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(&TR, A.x_toff + n, 8, cudaMemcpyDeviceToHost, st));
@@ -1482,7 +1508,7 @@ static int enqueue_paths_count(abb_graph *g, const abb_paths_io *io, cudaStream_
     PathsArgs A = paths_base(g);
     A.io = *io; A.f_cnt = g->pl_cnt.as<int64_t>(); A.f_link = g->pl_link.as<int2>(); A.f_lcnt = link_counts ? g->pl_lcnt.as<int64_t>() : nullptr;
     finding_rows_kernel<<<static_cast<unsigned>((nf + 1 + 255) / 256), 256, 0, st>>>(A); g_launches++;
-    if ((rc = scan_i64(g, A.f_cnt, io->f_off, nf + 1, st))) return rc;
+    if ((rc = scan_i64(g->p_scan_tmp, A.f_cnt, io->f_off, nf + 1, st))) return rc;
     CUDA_TRY(cudaGetLastError());
     g->paths_args = A;
     g->paths_args_valid = true;
@@ -1619,12 +1645,11 @@ static int paths_run(abb_graph *g, const int32_t *h_findings, const int32_t *d_f
     int rc = g->pl_off.ensure(static_cast<size_t>(nf + 1) * 8);
     if (rc) return rc;
     int64_t *link_off = g->pl_off.as<int64_t>();
-    if ((rc = scan_i64(g, A.f_lcnt, link_off, nf + 1, st))) return rc;
+    if ((rc = scan_i64(g->p_scan_tmp, A.f_lcnt, link_off, nf + 1, st))) return rc;
     int64_t NL = 0;
     CUDA_TRY(cudaMemcpyAsync(&NL, link_off + nf, 8, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     const int64_t nu_max = std::min<int64_t>(NL, n);
-#define ENS(buf, bytes) if (!rc) rc = g->buf.ensure(static_cast<size_t>(bytes))
     ENS(pl_vs, (NL + 2) * 4); ENS(pl_rel, NL + 16); ENS(pl_roff, (NL + 2) * 8); ENS(pl_toff, (NL + 2) * 8); ENS(pl_need, n + 16); ENS(pl_ulist, (n + 2) * 4);
     ENS(pl_nu, 16); ENS(pt_cnt, (nu_max + 2) * 8); ENS(pt_off, (nu_max + 2) * 8); ENS(pt_off_node, (n + 2) * 8);
     if (rc) return rc;
@@ -1635,22 +1660,14 @@ static int paths_run(abb_graph *g, const int32_t *h_findings, const int32_t *d_f
     unsigned long long *nu = g->pl_nu.as<unsigned long long>();
     CUDA_TRY(cudaMemsetAsync(need, 0, static_cast<size_t>(n) + 16, st));
     batch_links_kernel<<<static_cast<unsigned>((nf + 1 + 255) / 256), 256, 0, st>>>(A, link_off, link_vs, link_rel, link_roff, need); g_launches++;
-    {
-        cub::CountingInputIterator<int32_t> iota(0);
-        size_t tmp = 0;
-        CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, tmp, iota, need, ulist, nu, static_cast<int>(n), st));
-        if ((rc = g->p_scan_tmp.ensure(tmp + 16))) return rc;
-        CUDA_TRY(cub::DeviceSelect::Flagged(g->p_scan_tmp.p, tmp, iota, need, ulist, nu, static_cast<int>(n), st));
-        g_launches++;
-    }
+    if ((rc = select_flagged(g->p_scan_tmp, need, ulist, nu, static_cast<int>(n), st))) return rc;
     CUDA_TRY(cudaMemsetAsync(t_cnt, 0, static_cast<size_t>(nu_max + 2) * 8, st));
     if (nu_max) { batch_template_counts_kernel<<<static_cast<unsigned>((nu_max + 255) / 256), 256, 0, st>>>(A, ulist, nu, t_cnt); g_launches++; }
-    if ((rc = scan_i64(g, t_cnt, t_off, nu_max + 1, st))) return rc;
+    if ((rc = scan_i64(g->p_scan_tmp, t_cnt, t_off, nu_max + 1, st))) return rc;
     int64_t TR = 0;
     CUDA_TRY(cudaMemcpyAsync(&TR, t_off + nu_max, 8, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     ENS(pt_row, (TR + 2) * 16); ENS(pt_rel, (TR + 2) * 2);
-#undef ENS
     if (rc) return rc;
     int64_t *t_off_node = g->pt_off_node.as<int64_t>();
     if (nu_max) { batch_templates_kernel<<<warp_grid(g, nu_max), 256, 0, st>>>(A, ulist, nu, t_off, t_off_node, g->pt_row.as<int4>(), g->pt_rel.as<int8_t>()); g_launches++; }
@@ -1663,15 +1680,11 @@ static int paths_run(abb_graph *g, const int32_t *h_findings, const int32_t *d_f
     bool ok = r->off.alloc(n1 * 8) && r->link_off.alloc(n1 * 8) && r->link_vs.alloc(NL * 4) && r->link_rel.alloc(NL) && r->link_roff.alloc((NL + 1) * 8) &&
               r->link_toff.alloc(NL * 8) && r->t_row.alloc(TR * 16) && r->t_rel.alloc(TR * 2);
     if (!ok) return fail(ABB_ERR_NOMEM, "pinned host allocation failed");
-    cudaError_t e = cudaSuccess;
-    auto d2h = [&](HostBlock &dst, const void *src, size_t bytes) {
-        if (e == cudaSuccess && bytes) e = cudaMemcpyAsync(dst.p, src, bytes, cudaMemcpyDeviceToHost, st);
-        r->d2h += static_cast<int64_t>(bytes);
-    };
+    Readback d2h{st, &r->d2h};
     d2h(r->off, io.f_off, n1 * 8); d2h(r->link_off, link_off, n1 * 8); d2h(r->link_vs, link_vs, NL * 4); d2h(r->link_rel, link_rel, NL);
     d2h(r->link_roff, link_roff, (NL + 1) * 8); d2h(r->link_toff, link_toff, NL * 8); d2h(r->t_row, g->pt_row.p, TR * 16); d2h(r->t_rel, g->pt_rel.p, TR * 2);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) return fail(ABB_ERR_CUDA, "paths D2H failed: %s", cudaGetErrorString(e));
+    if (d2h.err == cudaSuccess) d2h.err = cudaStreamSynchronize(st);
+    if (d2h.err != cudaSuccess) return fail(ABB_ERR_CUDA, "paths D2H failed: %s", cudaGetErrorString(d2h.err));
     r->rows = r->off.as<int64_t>()[nf];
     *out = r.release();
     return ABB_OK;
@@ -1720,19 +1733,12 @@ static int paths_rank(abb_graph *g, const int32_t *findings, int64_t n_findings,
     if (int rc = g->p_findings.ensure(static_cast<size_t>(nf + 1) * 4)) return rc;
     if (int rc = g->p_off.ensure(static_cast<size_t>(nf + 1) * 8)) return rc;
     DevBuf d_base, d_tab, d_ncu, d_ntu, d_focus;
-    if (int rc = d_base.alloc(static_cast<size_t>(nf + 1) * 4)) return rc;
-    if (int rc = d_tab.alloc(static_cast<size_t>(n_base) * 75 * 4)) return rc;
-    if (int rc = d_ncu.alloc(static_cast<size_t>(n + 1) * 4)) return rc;
-    if (int rc = d_ntu.alloc(static_cast<size_t>(n + 1) * 4)) return rc;
-    if (focused) { if (int rc = d_focus.alloc(static_cast<size_t>(n + 1))) return rc; }
-    if (nf) {
-        CUDA_TRY(cudaMemcpyAsync(g->p_findings.p, findings, static_cast<size_t>(nf) * 4, cudaMemcpyHostToDevice, st));
-        CUDA_TRY(cudaMemcpyAsync(d_base.p, base_id, static_cast<size_t>(nf) * 4, cudaMemcpyHostToDevice, st));
-    }
-    CUDA_TRY(cudaMemcpyAsync(d_tab.p, risk_rank, static_cast<size_t>(n_base) * 75 * 4, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(d_ncu.p, ncu, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(d_ntu.p, ntu, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, st));
-    if (focused) CUDA_TRY(cudaMemcpyAsync(d_focus.p, node_focus, static_cast<size_t>(n), cudaMemcpyHostToDevice, st));
+    if (nf) CUDA_TRY(cudaMemcpyAsync(g->p_findings.p, findings, static_cast<size_t>(nf) * 4, cudaMemcpyHostToDevice, st));
+    if (int rc = d_base.upload(base_id, static_cast<size_t>(nf) * 4, st, 4)) return rc;
+    if (int rc = d_tab.upload(risk_rank, static_cast<size_t>(n_base) * 75 * 4, st)) return rc;
+    if (int rc = d_ncu.upload(ncu, static_cast<size_t>(n) * 4, st, 4)) return rc;
+    if (int rc = d_ntu.upload(ntu, static_cast<size_t>(n) * 4, st, 4)) return rc;
+    if (focused) { if (int rc = d_focus.upload(node_focus, static_cast<size_t>(n), st, 1)) return rc; }
     abb_paths_io io{};
     io.n_findings = nf; io.findings = g->p_findings.as<int32_t>(); io.f_off = g->p_off.as<int64_t>();
     if (int rc = enqueue_paths_count(g, &io, st)) return rc;
@@ -1745,7 +1751,7 @@ static int paths_rank(abb_graph *g, const int32_t *findings, int64_t n_findings,
     r->matched = R;
     // unfocused, the page is known before any kernel runs; focused, the matched count is needed first
     if (R == 0 || (!focused && std::min(limit, R - std::min(offset, R)) == 0)) { r->matched = focused ? 0 : R; *out = r.release(); return ABB_OK; }
-    DevBuf k1, k2, v1, v2, tmp, d_sel, sel_tmp;
+    DevBuf k1, k2, v1, v2, tmp, d_sel;
     int rc = k1.alloc(static_cast<size_t>(R) * 8);
     if (!rc) rc = k2.alloc(static_cast<size_t>(R) * 8);
     if (!rc) rc = v1.alloc(static_cast<size_t>(R) * 4);
@@ -1758,19 +1764,14 @@ static int paths_rank(abb_graph *g, const int32_t *findings, int64_t n_findings,
     // sort input: every row (k1, v1), or the matched rows compacted into (k2, v2); the sorted pairs land in the other pair
     unsigned long long *key_in = k1.as<unsigned long long>(), *key_out = k2.as<unsigned long long>();
     uint32_t *row_in = v1.as<uint32_t>(), *row_out = v2.as<uint32_t>();
-    cudaError_t ce = cudaSuccess;
-    size_t tb = 0;
     if (focused) {
-        if (!(rc = d_sel.alloc(8))) {
-            ce = cub::DeviceSelect::If(nullptr, tb, v1.as<uint32_t>(), v2.as<uint32_t>(), d_sel.as<int64_t>(), static_cast<int>(R), RowMatched{}, st);
-            if (ce == cudaSuccess && !(rc = sel_tmp.alloc(tb)))
-                ce = cub::DeviceSelect::If(sel_tmp.p, tb, v1.as<uint32_t>(), v2.as<uint32_t>(), d_sel.as<int64_t>(), static_cast<int>(R), RowMatched{}, st);
-            g_launches++;
-        }
+        if ((rc = d_sel.alloc(8))) return rc;
+        if ((rc = cub_run(tmp, [&](void *t, size_t &b) {
+                 return cub::DeviceSelect::If(t, b, v1.as<uint32_t>(), v2.as<uint32_t>(), d_sel.as<int64_t>(), static_cast<int>(R), RowMatched{}, st);
+             }))) return rc;
         int64_t M = 0;
-        if (!rc && ce == cudaSuccess) ce = cudaMemcpyAsync(&M, d_sel.p, 8, cudaMemcpyDeviceToHost, st);
-        if (!rc && ce == cudaSuccess) ce = cudaStreamSynchronize(st);
-        if (rc || ce != cudaSuccess) return rc ? rc : fail(ABB_ERR_CUDA, "focus compaction failed: %s", cudaGetErrorString(ce));
+        CUDA_TRY(cudaMemcpyAsync(&M, d_sel.p, 8, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
         r->matched = M;
         if (M == 0 || std::min(limit, M - std::min(offset, M)) == 0) { *out = r.release(); return ABB_OK; }
         gather_keys_kernel<<<static_cast<unsigned>((M + 255) / 256), 256, 0, st>>>(k1.as<unsigned long long>(), v2.as<uint32_t>(), M, k2.as<unsigned long long>());
@@ -1780,12 +1781,8 @@ static int paths_rank(abb_graph *g, const int32_t *findings, int64_t n_findings,
     const int64_t M = r->matched;
     const int64_t first = std::min(offset, M), count = std::min(limit, M - first);
     r->count = count;
-    tb = 0;
-    ce = cub::DeviceRadixSort::SortPairs(nullptr, tb, key_in, key_out, row_in, row_out, static_cast<int>(M), 0, 64, st);
-    if (ce == cudaSuccess && !(rc = tmp.alloc(tb)))
-        ce = cub::DeviceRadixSort::SortPairs(tmp.p, tb, key_in, key_out, row_in, row_out, static_cast<int>(M), 0, 64, st);
-    g_launches++;
-    if (rc || ce != cudaSuccess) return rc ? rc : fail(ABB_ERR_CUDA, "radix sort failed: %s", cudaGetErrorString(ce));
+    if ((rc = cub_run(tmp, [&](void *t, size_t &b) { return cub::DeviceRadixSort::SortPairs(t, b, key_in, key_out, row_in, row_out, static_cast<int>(M), 0, 64, st); })))
+        return rc;
     DevBuf o_hops, o_rels, o_nc, o_nt, o_rank, o_row;
     rc = o_hops.alloc(static_cast<size_t>(count) * 16);
     if (!rc) rc = o_rels.alloc(static_cast<size_t>(count) * 4);
@@ -1799,7 +1796,7 @@ static int paths_rank(abb_graph *g, const int32_t *findings, int64_t n_findings,
     g_launches++;
     r->hops.resize(static_cast<size_t>(count) * 4); r->rels.resize(static_cast<size_t>(count) * 4); r->ncred.resize(count); r->ntool.resize(count);
     r->risk_rank.resize(count); r->row.resize(count);
-    ce = cudaGetLastError();
+    cudaError_t ce = cudaGetLastError();
     if (ce == cudaSuccess) ce = cudaMemcpyAsync(r->hops.data(), o_hops.p, static_cast<size_t>(count) * 16, cudaMemcpyDeviceToHost, st);
     if (ce == cudaSuccess) ce = cudaMemcpyAsync(r->rels.data(), o_rels.p, static_cast<size_t>(count) * 4, cudaMemcpyDeviceToHost, st);
     if (ce == cudaSuccess) ce = cudaMemcpyAsync(r->ncred.data(), o_nc.p, static_cast<size_t>(count) * 4, cudaMemcpyDeviceToHost, st);
@@ -1911,7 +1908,6 @@ extern "C" int abb_finding_context_host(abb_graph *g, int32_t max_depth, const i
     const size_t q = static_cast<size_t>(nq), q1 = q + 1;
     auto drain = [&]() { cudaStreamSynchronize(st); cudaStreamSynchronize(cs); };
     int rc = ABB_OK;
-#define ENS(buf, bytes) if (!rc) rc = g->buf.ensure(static_cast<size_t>(bytes))
     ENS(d_roots, q1 * 4); ENS(cx_bcnt, q1 * CTX_BUCKETS * 4); ENS(cx_cnt, q1 * 8); ENS(cx_start, q1 * 8);
     if (rc) return rc;
     std::unique_ptr<abb_finding_context_result> r(new abb_finding_context_result());
@@ -1928,7 +1924,7 @@ extern "C" int abb_finding_context_host(abb_graph *g, int32_t max_depth, const i
     CUDA_TRY(cudaEventRecord(g->cx_ev[0], cs));
     CUDA_TRY(cudaMemsetAsync(A.cnt, 0, q1 * 8, cs));
     if (nq) { context_kernel<false><<<grid, 256, 0, cs>>>(A); g_launches++; }
-    if ((rc = scan_i64(g, A.cnt, g->cx_start.as<int64_t>(), nq + 1, cs))) { drain(); return rc; }
+    if ((rc = scan_i64(g->p_scan_tmp, A.cnt, g->cx_start.as<int64_t>(), nq + 1, cs))) { drain(); return rc; }
     CUDA_TRY(cudaEventRecord(g->cx_ev[1], cs));
     // the impact walk, unchanged, into the device arena
     const abb_walk_spec spec = abb_spec_impact_of(max_depth);
@@ -1940,7 +1936,6 @@ extern "C" int abb_finding_context_host(abb_graph *g, int32_t max_depth, const i
     CUDA_TRY(cudaStreamSynchronize(cs));
     r->total = total;
     ENS(cx_src, (total + 1) * 4);
-#undef ENS
     if (rc) { drain(); return rc; }
     if (!(r->start.alloc(q * 8) && r->bcnt.alloc(q * CTX_BUCKETS * 4) && r->src.alloc(static_cast<size_t>(total) * 4))) {
         drain(); return fail(ABB_ERR_NOMEM, "pinned host allocation failed");
@@ -1950,12 +1945,9 @@ extern "C" int abb_finding_context_host(abb_graph *g, int32_t max_depth, const i
     CUDA_TRY(cudaEventRecord(g->cx_ev[2], cs));
     if (nq) { context_kernel<true><<<grid, 256, 0, cs>>>(A); g_launches++; }
     CUDA_TRY(cudaEventRecord(g->cx_ev[3], cs));
-    cudaError_t e = cudaGetLastError();
-    auto d2h = [&](HostBlock &dst, const void *src, size_t bytes) {
-        r->d2h += static_cast<int64_t>(bytes);
-        if (e == cudaSuccess && bytes) e = cudaMemcpyAsync(dst.p, src, bytes, cudaMemcpyDeviceToHost, cs);
-    };
+    Readback d2h{cs, &r->d2h, cudaGetLastError()};
     d2h(r->start, g->cx_start.p, q * 8); d2h(r->bcnt, g->cx_bcnt.p, q * CTX_BUCKETS * 4); d2h(r->src, g->cx_src.p, static_cast<size_t>(total) * 4);
+    cudaError_t e = d2h.err;
     if (e != cudaSuccess) { drain(); return fail(ABB_ERR_CUDA, "finding context failed: %s", cudaGetErrorString(e)); }
     abb_walk_result *walk = nullptr;
     if ((rc = walk_collect(g, &spec, io, totals, wh2d, &walk, true, nullptr, false))) { drain(); return rc; }
