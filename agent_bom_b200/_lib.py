@@ -210,6 +210,12 @@ EXPORTS = {
     "abb_delta_build_host": (C.c_int, [vp, vp, vp, vp, vp, vp]),
     "abb_delta_result_free": (None, [vp]),
     "abb_delta_fetch_host": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "abb_lookup_table_host": (C.c_int, [vp, i32, vp, i64, vp, vp, vp, vp]),
+    "abb_lookup_table_bytes": (i64, [vp]),
+    "abb_lookup_edges_host": (C.c_int, [vp, i64, vp, vp, vp]),
+    "abb_lookup_context_host": (C.c_int, [vp, i32, vp, vp]),
+    "abb_lookup_fetch_host": (C.c_int, [vp, vp]),
+    "abb_lookup_result_free": (None, [vp]),
 }
 
 _lock = threading.Lock()

@@ -34,6 +34,7 @@
 #include "delta.cuh"
 #include "walk.cuh"
 #include "walkb.cuh"
+#include "lookup.cuh"
 
 using namespace abb;
 
@@ -353,6 +354,11 @@ struct abb_graph {
     int64_t dl_ne = 0;
     bool dl_has_w = false;
     int64_t dl_union_limit = DL_UNION_LIMIT;
+    // lookup table (lookup_host.inl): per original edge the rank of its relationship string among the graph's.  lk_ready = false until built.
+    // The lookup workspace (node list, entry offsets, edge bitmap and its scan, context keys, counter, cub temp) is reused under mu.
+    DevBuf lk_erel;
+    bool lk_ready = false;
+    DevBuf lk_nodes, lk_start, lk_bits, lk_cnt, lk_off, lk_keys, lk_keys2, lk_vals, lk_ctr, lk_tmp;
     // graph arrays of an uploaded graph (an adopted graph's belong to the caller)
     std::vector<DevBuf> owned_arrays;
 
@@ -1968,3 +1974,4 @@ extern "C" int abb_finding_context_host(abb_graph *g, int32_t max_depth, const i
 #include "lateral_host.inl"
 #include "clusters_host.inl"
 #include "delta_host.inl"
+#include "lookup_host.inl"

@@ -624,6 +624,47 @@ class DeviceGraph:
             lib.abb_delta_result_free(res)
         return out
 
+    def build_lookup_table(self, n_real: int, severity, erel) -> dict[str, np.ndarray]:
+        """Store the graph's lookup table (``abb_lookup_table_host``), replacing an earlier one, and return the snapshot statistics:
+        ``type`` [256] and ``severity`` [256] counts of the real nodes by code, ``relationship`` [64] counts of the original edges
+        between real nodes by ``erel``.  ``severity``: a code per real node; ``erel``: per original edge, the rank (< 64) of its
+        relationship string among the graph's."""
+        severity = np.ascontiguousarray(severity, np.uint8)
+        erel = np.ascontiguousarray(erel, np.uint8)
+        if severity.shape != (n_real,) or not 0 <= n_real <= self.n_nodes or erel.ndim != 1 or erel.shape[0] > self.n_entries:
+            raise ValueError("lookup table inputs have the wrong shapes")
+        out = {"type": np.zeros(256, np.int64), "severity": np.zeros(256, np.int64), "relationship": np.zeros(64, np.int64)}
+        with self._use() as h:
+            _lib.check(_lib.load().abb_lookup_table_host(h, n_real, severity.ctypes.data, erel.shape[0], erel.ctypes.data,
+                                                         *(out[k].ctypes.data for k in ("type", "severity", "relationship"))))
+        return out
+
+    def lookup_table_bytes(self) -> int:
+        with self._use() as h:
+            return int(_lib.load().abb_lookup_table_bytes(h))
+
+    def _lookup(self, build) -> np.ndarray:
+        lib = _lib.load()
+        res, count = _vp(), C.c_int64(0)
+        with self._use() as h:
+            _lib.check(build(lib, h, C.byref(res), C.byref(count)))
+        try:
+            out = np.empty(count.value, np.int32)
+            _lib.check(lib.abb_lookup_fetch_host(res, out.ctypes.data))
+        finally:
+            lib.abb_lookup_result_free(res)
+        return out
+
+    def incident_edges(self, nodes) -> np.ndarray:
+        """Original edges with at least one endpoint in ``nodes``, ascending (``abb_lookup_edges_host``)."""
+        nodes = _i32(nodes)
+        return self._lookup(lambda lib, h, res, cnt: lib.abb_lookup_edges_host(h, nodes.shape[0], nodes.ctypes.data, res, cnt))
+
+    def context_edges(self, node: int) -> np.ndarray:
+        """Original edges incident to ``node`` in (source rank, target rank, relationship rank) order (``abb_lookup_context_host``);
+        needs the lookup table."""
+        return self._lookup(lambda lib, h, res, cnt: lib.abb_lookup_context_host(h, int(node), res, cnt))
+
     def betweenness(self) -> np.ndarray:
         """``nx.betweenness_centrality`` of the graph as a DiGraph (``abb_betweenness_host``): f64 per node."""
         out = np.zeros(self.n_nodes, dtype=np.float64)

@@ -72,6 +72,7 @@ class UnifiedGraph:
         self._edge_lookup = None
         self._clusters = None              # semantic-cluster key table (graph/clusters.py)
         self._delta = None                 # snapshot-diff tables (graph/delta.py)
+        self._lookup = None                # snapshot-lookup table and statistics (graph/lookup.py)
 
     # ── construction from foreign graphs ────────────────────────────────
     @classmethod
@@ -91,7 +92,7 @@ class UnifiedGraph:
     # ── mutation (reference container.py:116-198) ───────────────────────
     def _invalidate(self) -> None:
         self._csr = None
-        self._rank_inputs = self._focus_index = self._edge_lookup = self._clusters = self._delta = None
+        self._rank_inputs = self._focus_index = self._edge_lookup = self._clusters = self._delta = self._lookup = None
         if self._dg is not None:
             self._dg.close()
             self._dg = None

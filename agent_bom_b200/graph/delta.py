@@ -54,34 +54,49 @@ def _pack(strings) -> tuple[bytes, np.ndarray]:
     return b"".join(enc), off
 
 
+def real_records(graph) -> list:
+    """The node records of the graph's real nodes, in index order."""
+    nodes = graph.nodes
+    return [nodes[nid] for nid in graph.csr.node_ids[:graph.csr.n_real]]
+
+
+def severity_codes(recs) -> np.ndarray:
+    """``SEVERITY_CODES`` of each record's severity string; ``CODE_OTHER`` for a string outside the table."""
+    return np.fromiter((SEVERITY_CODES.get(r.severity or "", CODE_OTHER) for r in recs), np.uint8, len(recs))
+
+
+def relationship_slots(graph) -> tuple[np.ndarray, list[str]]:
+    """Per original edge the slot of its relationship string, and the graph's distinct relationship strings in sorted order (the
+    slot is the string's rank).  More than ``REL_SLOTS`` strings is an error."""
+    codes = np.asarray(graph.csr.rel, np.int64)
+    other = {int(i): enum_value(graph.edges[int(i)].relationship) for i in np.flatnonzero(codes == REL_CODE_OTHER)}
+    names = sorted({RELATIONSHIP_VALUES[c] for c in np.unique(codes).tolist() if c != REL_CODE_OTHER} | set(other.values()))
+    if len(names) > REL_SLOTS:
+        raise ValueError(f"{len(names)} distinct relationships exceed the {REL_SLOTS} relationship slots")
+    slot = {s: i for i, s in enumerate(names)}
+    code_slot = np.zeros(32, np.uint8)
+    for c, v in enumerate(RELATIONSHIP_VALUES):
+        code_slot[c] = slot.get(v, 0)
+    erel = code_slot[codes] if codes.size else np.zeros(0, np.uint8)
+    for i, v in other.items():
+        erel[i] = slot[v]
+    return erel, names
+
+
 class DeltaTable:
     """Host half of a graph's diff tables: the relationship strings of its slots, and the per-graph arrays uploaded once."""
 
     def __init__(self, graph):
         csr = graph.csr
         n_real = csr.n_real
-        nodes = graph.nodes
-        recs = [nodes[nid] for nid in csr.node_ids[:n_real]]
+        recs = real_records(graph)
         self.ids_bytes, self.id_off = _pack(csr.node_ids)
         self.perm = np.argsort(csr.node_rank, kind="stable").astype(np.int32)
         self.label_bytes, self.label_off = _pack([_text(r.label) for r in recs])
         self.status = np.fromiter((STATUS_CODES.get(_text(r.status), CODE_OTHER) for r in recs), np.uint8, n_real)
-        self.severity = np.fromiter((SEVERITY_CODES.get(r.severity or "", CODE_OTHER) for r in recs), np.uint8, n_real)
+        self.severity = severity_codes(recs)
         self.risk = np.fromiter((_risk(r.risk_score) for r in recs), np.float64, n_real)
-        # relationship slots: this graph's distinct relationship strings in sorted order
-        codes = np.asarray(csr.rel, np.int64)
-        other = {int(i): enum_value(graph.edges[int(i)].relationship) for i in np.flatnonzero(codes == REL_CODE_OTHER)}
-        names = sorted({RELATIONSHIP_VALUES[c] for c in np.unique(codes).tolist() if c != REL_CODE_OTHER} | set(other.values()))
-        if len(names) > REL_SLOTS:
-            raise ValueError(f"{len(names)} distinct relationships exceed the diff's {REL_SLOTS}")
-        slot = {s: i for i, s in enumerate(names)}
-        code_slot = np.zeros(32, np.uint8)
-        for c, v in enumerate(RELATIONSHIP_VALUES):
-            code_slot[c] = slot.get(v, 0)
-        self.erel = code_slot[codes] if codes.size else np.zeros(0, np.uint8)
-        for i, v in other.items():
-            self.erel[i] = slot[v]
-        self.rel_names = names
+        self.erel, self.rel_names = relationship_slots(graph)
         self.eflag = np.ascontiguousarray(csr.flags, np.uint8)
         self.uploaded = False
 

@@ -143,6 +143,25 @@ class SnapshotNode:
         return d
 
 
+def node_columns(values) -> dict[str, Any]:
+    """The lazy columns of a node row (``_NODE_LAZY_COLUMNS`` order), JSON decoded as the reference's ``_node_from_row`` does."""
+    full = dict(zip(_NODE_LAZY_COLUMNS, values))
+    for c in _NODE_JSON_COLUMNS:
+        full[c] = json.loads(full[c]) if full[c] else ({} if c in ("attributes", "dimensions") else [])
+    return full
+
+
+_EDGE_LAZY_COLUMNS = ("first_seen", "last_seen", "valid_from", "valid_to", "confidence", "provenance", "source_scan_id", "source_run_id", "evidence", "activity_id")
+
+
+def edge_columns(values, scan_id: str) -> dict[str, Any]:
+    """The lazy columns of an edge row (``_EDGE_LAZY_COLUMNS`` order) as the reference's ``_edge_from_row`` reads them."""
+    first_seen, last_seen, valid_from, valid_to, confidence, provenance, src_scan, src_run, evidence, activity = values
+    return {"first_seen": first_seen, "last_seen": last_seen, "valid_from": valid_from or first_seen, "valid_to": valid_to,
+            "confidence": confidence, "provenance": json.loads(provenance or "{}"), "source_scan_id": src_scan or scan_id,
+            "source_run_id": src_run or "", "evidence": json.loads(evidence or "{}"), "activity_id": activity}
+
+
 class SnapshotEdge:
     """Edge record synthesised from the edge arrays; evidence / provenance / timestamps are read on first use."""
 
@@ -263,14 +282,9 @@ class SnapshotGraph(UnifiedGraph):
                 q = (f"SELECT id, {', '.join(_NODE_LAZY_COLUMNS)} FROM graph_nodes WHERE tenant_id = ? AND scan_id = ? "
                      f"AND id IN ({','.join('?' * len(chunk))})")
                 for row in conn.execute(q, [tenant, self.scan_id, *chunk]):
-                    full = dict(zip(_NODE_LAZY_COLUMNS, row[1:]))
-                    for c in _NODE_JSON_COLUMNS:
-                        full[c] = json.loads(full[c]) if full[c] else ({} if c in ("attributes", "dimensions") else [])
-                    self.nodes[row[0]]._full = full
+                    self.nodes[row[0]]._full = node_columns(row[1:])
         finally:
             conn.close()
-
-    _EDGE_LAZY_COLUMNS = ("first_seen", "last_seen", "valid_from", "valid_to", "confidence", "provenance", "source_scan_id", "source_run_id", "evidence", "activity_id")
 
     def hydrate_edges(self, edges) -> None:
         """Read the wide columns of the given edge records, 250 rows per query."""
@@ -286,16 +300,13 @@ class SnapshotGraph(UnifiedGraph):
         try:
             for a in range(0, len(keys), 250):
                 chunk = keys[a: a + 250]
-                q = (f"SELECT source_id, target_id, relationship, {', '.join(self._EDGE_LAZY_COLUMNS)} FROM graph_edges WHERE tenant_id = ? AND scan_id = ? "
+                q = (f"SELECT source_id, target_id, relationship, {', '.join(_EDGE_LAZY_COLUMNS)} FROM graph_edges WHERE tenant_id = ? AND scan_id = ? "
                      f"AND (source_id, target_id, relationship) IN (VALUES {','.join(['(?,?,?)'] * len(chunk))})")
                 params = [tenant, self.scan_id]
                 for k in chunk:
                     params.extend(k)
                 for row in conn.execute(q, params):
-                    first_seen, last_seen, valid_from, valid_to, confidence, provenance, src_scan, src_run, evidence, activity = row[3:]
-                    full = {"first_seen": first_seen, "last_seen": last_seen, "valid_from": valid_from or first_seen, "valid_to": valid_to,
-                            "confidence": confidence, "provenance": json.loads(provenance or "{}"), "source_scan_id": src_scan or self.scan_id,
-                            "source_run_id": src_run or "", "evidence": json.loads(evidence or "{}"), "activity_id": activity}
+                    full = edge_columns(row[3:], self.scan_id)
                     for e in by_row.get((row[0], row[1], row[2]), ()):
                         e._full = full
         finally:

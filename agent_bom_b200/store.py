@@ -128,8 +128,8 @@ class B200GraphStore:
         if g is None or not g.has_node(source):
             return [], set()
         paths = g.bfs(source, max_depth=max_depth, traversable_only=traversable_only)
-        reachable = g.reachable_from(source, max_depth=max_depth, traversable_only=traversable_only, include_source=False)
-        return paths, reachable
+        # under the same depth and traversable flag, the BFS paths end at exactly the nodes reachable_from(include_source=False) returns
+        return paths, {p[-1] for p in paths}
 
     def impact_of(self, *, tenant_id: str = "", scan_id: str = "", node_id: str, max_depth: int = 4) -> dict[str, Any] | None:
         g = self._graph(tenant_id, scan_id)
@@ -235,6 +235,105 @@ class B200GraphStore:
             return g if g is not None else UnifiedGraph(scan_id=scan_id, tenant_id=tenant, device=self._device)
 
         return snapshot_diff(snapshot(scan_id_old), snapshot(scan_id_new), db_path=db_path, tenant_id=tenant)
+
+    # ── record lookups (GPU over the snapshot cache; SQLite only by key) ──
+    def _sqlite_db(self) -> str | None:
+        """The inner store's database file when it is SQLite-backed (``_db_path``, as for topology-first loading), else ``None``."""
+        from pathlib import Path
+
+        db_path = getattr(self._inner, "_db_path", None) if self._inner is not None else None
+        return str(db_path) if db_path is not None and Path(db_path).exists() else None
+
+    def _delegate(self, name: str, **kwargs):
+        inner = getattr(self._inner, name, None) if self._inner is not None else None
+        if inner is None:
+            raise B200UnsupportedOperationError(f"B200GraphStore has no inner store to serve {name}()")
+        return inner(**kwargs)
+
+    def _snapshot(self, db_path: str, tenant_id: str, scan_id: str) -> UnifiedGraph | None:
+        """The cached graph of ``scan_id or`` the tenant's latest snapshot, resolved as the SQLite store does."""
+        if not scan_id:
+            from .graph.lookup import connect
+            from .graph.snapshot import latest_snapshot_id
+
+            conn = connect(db_path)
+            try:
+                scan_id = latest_snapshot_id(conn, tenant_id=tenant_id)
+            finally:
+                conn.close()
+            if not scan_id:
+                return None
+        return self._graph(tenant_id, scan_id)
+
+    def nodes_by_ids(self, *, tenant_id: str = "", scan_id: str = "", node_ids: set[str]) -> list:
+        """Records of the ids that are nodes of the snapshot, in id order (reference api/graph_store.py:500-531)."""
+        db = self._sqlite_db()
+        if db is None:
+            return self._delegate("nodes_by_ids", tenant_id=tenant_id, scan_id=scan_id, node_ids=node_ids)
+        from .graph.lookup import nodes_by_ids
+
+        g = self._snapshot(db, tenant_id, scan_id) if node_ids else None
+        return [] if g is None else nodes_by_ids(g, db, normalize_tenant(tenant_id), node_ids)
+
+    def edges_for_node_ids(self, *, tenant_id: str = "", scan_id: str = "", node_ids: set[str]) -> list:
+        """Stored edge rows with an endpoint in ``node_ids``, in rowid order (reference api/graph_store.py:1315-1344).  The reference
+        binds two parameters per id and raises SQLite's too-many-variables error above about 16 000 ids; this store answers."""
+        db = self._sqlite_db()
+        if db is None:
+            return self._delegate("edges_for_node_ids", tenant_id=tenant_id, scan_id=scan_id, node_ids=node_ids)
+        from .graph.lookup import edges_for_node_ids
+
+        g = self._snapshot(db, tenant_id, scan_id) if node_ids else None
+        return [] if g is None else edges_for_node_ids(g, db, normalize_tenant(tenant_id), node_ids)
+
+    def node_context(self, *, tenant_id: str = "", scan_id: str = "", node_id: str) -> dict[str, Any] | None:
+        """The node record, its edges out and in (a bidirectional row adds its reversed copy to the other side), its neighbours and
+        sources, and ``impact_of`` (reference api/graph_store.py:889-948).  ``impact`` is the device walk over every stored row of the
+        snapshot, rows to ids that are not nodes included, so it equals the SQLite store's except where that store's 5 000-node /
+        25 000-edge walk caps truncate it."""
+        db = self._sqlite_db()
+        if db is None:
+            return self._delegate("node_context", tenant_id=tenant_id, scan_id=scan_id, node_id=node_id)
+        from .graph.container import reversed_edge
+        from .graph.lookup import node_context_edges, node_impact, nodes_by_ids
+
+        tenant = normalize_tenant(tenant_id)
+        g = self._snapshot(db, tenant_id, scan_id)
+        if g is None or not g.has_node(node_id):
+            return None
+        nodes = nodes_by_ids(g, db, tenant, {node_id})
+        if not nodes:
+            return None
+        edges_out: list = []
+        edges_in: list = []
+        neighbors: list[str] = []
+        sources: list[str] = []
+        for edge in node_context_edges(g, db, tenant, node_id):
+            if edge.source == node_id:
+                edges_out.append(edge)
+                neighbors.append(edge.target)
+                if edge.is_bidirectional:
+                    edges_in.append(reversed_edge(edge))
+                    sources.append(edge.target)
+            if edge.target == node_id:
+                edges_in.append(edge)
+                sources.append(edge.source)
+                if edge.is_bidirectional:
+                    edges_out.append(reversed_edge(edge))
+                    neighbors.append(edge.source)
+        return {"node": nodes[0], "edges_out": edges_out, "edges_in": edges_in, "neighbors": neighbors, "sources": sources,
+                "impact": node_impact(g, db, tenant, node_id)}
+
+    def snapshot_stats(self, *, tenant_id: str = "", scan_id: str = "", entity_types: set[str] | None = None, min_severity_rank: int = 0) -> dict[str, Any]:
+        """Node, edge, attack-path and interaction-risk statistics of the snapshot (reference api/graph_store.py:1139-1240).  Unfiltered
+        statistics come from the device once per graph; filtered ones from the inner store."""
+        db = self._sqlite_db()
+        if db is None or entity_types or min_severity_rank:
+            return self._delegate("snapshot_stats", tenant_id=tenant_id, scan_id=scan_id, entity_types=entity_types, min_severity_rank=min_severity_rank)
+        from .graph.lookup import EMPTY_STATS, snapshot_stats
+
+        g = self._snapshot(db, tenant_id, scan_id)
+        return dict(EMPTY_STATS) if g is None else snapshot_stats(g)
 
     # ── everything else: the wrapped default store ──────────────────────
     def __getattr__(self, name: str):

@@ -525,6 +525,27 @@ void abb_delta_result_free(abb_delta_result *r);
 int abb_delta_fetch_host(const abb_delta_result *r, int32_t *nodes_added, int32_t *nodes_removed, int32_t *changed_new, int32_t *changed_old,
                          uint8_t *changed_flag, int32_t *edges_added, int32_t *edges_removed, int32_t *echanged_new, int32_t *echanged_old);
 
+/* ---- snapshot lookups -----------------------------------------------------------------------------------------
+ * Replace the per-request edge-row scans of edges_for_node_ids, node_context and the unfiltered snapshot_stats
+ * (agent_bom/api/graph_store.py:889-948, 1139-1240, 1315-1344).  abb_lookup_table_host stores the graph's lookup table
+ * (replacing an earlier one; freed with the graph): erel[n_edges] is, per original edge in graph.edges order (every edge of
+ * the graph), the rank (< 64) of its relationship string among the graph's relationship strings.  It also writes the snapshot
+ * statistics: type_counts_out[256] counts the real nodes (index < n_real) by entity-type code, sev_counts_out[256] by the
+ * caller's severity[n_real] code, and rel_counts_out[64] the original edges whose endpoints are both real nodes by erel.
+ * abb_lookup_edges_host finds the original edges with at least one endpoint among nodes[k] (duplicates allowed) and
+ * abb_lookup_context_host those of one node, sorted by (rank(source), rank(target), erel); the context needs the lookup table
+ * and fails when the graph has more than 2^27 nodes.  Both answers stay on the device in *out, owned by the caller, so lookups
+ * may run concurrently on one graph; *count_out is the number of edges.  abb_lookup_fetch_host copies the edge indices (the
+ * edge set ascending, the context in its order).  All pointers are host memory. */
+int abb_lookup_table_host(abb_graph *g, int32_t n_real, const uint8_t *severity, int64_t n_edges, const uint8_t *erel, int64_t *type_counts_out,
+                          int64_t *sev_counts_out, int64_t *rel_counts_out);
+int64_t abb_lookup_table_bytes(const abb_graph *g);              /* device bytes of the lookup table, 0 when none */
+typedef struct abb_lookup_result abb_lookup_result;
+int abb_lookup_edges_host(abb_graph *g, int64_t k, const int32_t *nodes, abb_lookup_result **out, int64_t *count_out);
+int abb_lookup_context_host(abb_graph *g, int32_t node, abb_lookup_result **out, int64_t *count_out);
+int abb_lookup_fetch_host(const abb_lookup_result *r, int32_t *edges_out);
+void abb_lookup_result_free(abb_lookup_result *r);
+
 #ifdef __cplusplus
 }
 #endif
