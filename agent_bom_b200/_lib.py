@@ -52,6 +52,14 @@ class WalkIO(C.Structure):
     ]
 
 
+class SearchSpec(C.Structure):
+    _fields_ = [
+        ("mode", i32), ("n_patterns", i32), ("patterns", vp), ("pattern_off", vp), ("type_ok", vp), ("cmp_ok", vp), ("src_ok", vp),
+        ("n_types", i32), ("n_cmp", i32), ("n_src", i32), ("use_min_rank", i32), ("min_rank", i64), ("has_cursor", i32), ("cur_risk_null", i32),
+        ("cur_sev", i64), ("cur_risk", C.c_double), ("cur_label_gt", i64), ("cur_label_eq", i64), ("cur_id_gt", i64), ("offset", i64), ("take", i64),
+    ]
+
+
 class PathsIO(C.Structure):
     _fields_ = [
         ("n_findings", i64), ("findings", vp), ("f_off", vp), ("hops", vp), ("rels", vp), ("ncred", vp), ("ntool", vp), ("row_cap", i64),
@@ -216,6 +224,12 @@ EXPORTS = {
     "abb_lookup_context_host": (C.c_int, [vp, i32, vp, vp]),
     "abb_lookup_fetch_host": (C.c_int, [vp, vp]),
     "abb_lookup_result_free": (None, [vp]),
+    "abb_search_text_host": (C.c_int, [vp, i32, vp, vp, vp]),
+    "abb_search_table_host": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32]),
+    "abb_search_table_bytes": (i64, [vp]),
+    "abb_search_host": (C.c_int, [vp, vp, vp, vp, vp, vp]),
+    "abb_search_fetch_host": (C.c_int, [vp, vp]),
+    "abb_search_result_free": (None, [vp]),
 }
 
 _lock = threading.Lock()

@@ -35,6 +35,7 @@
 #include "walk.cuh"
 #include "walkb.cuh"
 #include "lookup.cuh"
+#include "search.cuh"
 
 using namespace abb;
 
@@ -359,6 +360,15 @@ struct abb_graph {
     DevBuf lk_erel;
     bool lk_ready = false;
     DevBuf lk_nodes, lk_start, lk_bits, lk_cnt, lk_off, lk_keys, lk_keys2, lk_vals, lk_ctr, lk_tmp;
+    // search table (search_host.inl): per node the raw and token text with offsets, the rows a warp does not scan, severity, risk,
+    // label rank, entity-type / compliance / data-source codes, and the page order with its inverse.  sr_ready = false until built;
+    // sr_n = -1 until the text is stored.  The search workspace (flags, selection, counters, patterns and tables, cub temp) is
+    // reused under mu.
+    DevBuf sr_raw, sr_roff, sr_tok, sr_toff, sr_long, sr_sev, sr_risk, sr_label, sr_type, sr_cmp, sr_src, sr_order, sr_pos;
+    int32_t sr_n = -1, sr_types = 0, sr_ncmp = 0, sr_nsrc = 0;
+    int64_t sr_n_long = 0;
+    bool sr_ready = false;
+    DevBuf sr_flags, sr_sel, sr_ctr, sr_pat, sr_tmp;
     // graph arrays of an uploaded graph (an adopted graph's belong to the caller)
     std::vector<DevBuf> owned_arrays;
 
@@ -1975,3 +1985,4 @@ extern "C" int abb_finding_context_host(abb_graph *g, int32_t max_depth, const i
 #include "clusters_host.inl"
 #include "delta_host.inl"
 #include "lookup_host.inl"
+#include "search_host.inl"

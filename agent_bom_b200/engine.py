@@ -665,6 +665,65 @@ class DeviceGraph:
         needs the lookup table."""
         return self._lookup(lambda lib, h, res, cnt: lib.abb_lookup_context_host(h, int(node), res, cnt))
 
+    def search_text(self, text_off, text: bytes) -> np.ndarray:
+        """Store the search table's raw text, one row per node in id order (``abb_search_text_host``), and return the code points
+        >= 0x80 it holds, ascending."""
+        text_off = np.ascontiguousarray(text_off, np.int64)
+        buf = np.frombuffer(text, np.uint8) if text else np.zeros(1, np.uint8)
+        if text_off.ndim != 1 or text_off.shape[0] < 1 or int(text_off[-1]) != len(text):
+            raise ValueError("search text offsets do not match the text")
+        bits = np.zeros(0x110000 // 32, np.uint32)
+        with self._use() as h:
+            _lib.check(_lib.load().abb_search_text_host(h, text_off.shape[0] - 1, text_off.ctypes.data, buf.ctypes.data, bits.ctypes.data))
+        return np.flatnonzero(np.unpackbits(bits.view(np.uint8), bitorder="little"))
+
+    def build_search_table(self, fold, severity, risk, label_rank, type_code, cmp_code, src_code, n_types: int, n_cmp: int, n_src: int) -> None:
+        """Fold the stored text into token text and store the search table's keys and page order (``abb_search_table_host``);
+        freed with the graph.  ``fold`` [0x110000]: -1 separator, 0 folds away, else the folded code point."""
+        fold = np.ascontiguousarray(fold, np.int32)
+        severity, type_code, cmp_code, src_code = (_i32(a) for a in (severity, type_code, cmp_code, src_code))
+        risk = np.ascontiguousarray(risk, np.float64)
+        label_rank = np.ascontiguousarray(label_rank, np.uint32)
+        n = severity.shape[0]
+        if fold.shape != (0x110000,) or any(a.shape != (n,) for a in (risk, label_rank, type_code, cmp_code, src_code)):
+            raise ValueError("search table inputs have the wrong shapes")
+        with self._use() as h:
+            _lib.check(_lib.load().abb_search_table_host(h, fold.ctypes.data, severity.ctypes.data, risk.ctypes.data, label_rank.ctypes.data,
+                                                         type_code.ctypes.data, cmp_code.ctypes.data, src_code.ctypes.data, n_types, n_cmp, n_src))
+
+    def search_table_bytes(self) -> int:
+        with self._use() as h:
+            return int(_lib.load().abb_search_table_bytes(h))
+
+    def search(self, mode: int, patterns: list[bytes], type_ok=None, cmp_ok=None, src_ok=None, min_rank: int | None = None, cursor=None,
+               offset: int = 0, take: int = -1) -> tuple[np.ndarray, int, int]:
+        """One search or page call (``abb_search_host``): ``(page, total, selected)``, the page being node indices in page order.
+        ``cursor``: ``(severity, risk or None, label_gt, label_eq, id_gt)`` as abb200.h describes; ``take`` < 0: to the end."""
+        off = np.zeros(len(patterns) + 1, np.int64)
+        off[1:] = np.cumsum([len(p) for p in patterns])
+        blob = np.frombuffer(b"".join(patterns) or b"\0", np.uint8)
+        tabs = [None if t is None else np.ascontiguousarray(t, np.uint8) for t in (type_ok, cmp_ok, src_ok)]
+        spec = _lib.SearchSpec(mode=mode, n_patterns=len(patterns), patterns=blob.ctypes.data, pattern_off=off.ctypes.data,
+                               type_ok=None if tabs[0] is None else tabs[0].ctypes.data, cmp_ok=None if tabs[1] is None else tabs[1].ctypes.data,
+                               src_ok=None if tabs[2] is None else tabs[2].ctypes.data,
+                               n_types=0 if tabs[0] is None else tabs[0].shape[0], n_cmp=0 if tabs[1] is None else tabs[1].shape[0],
+                               n_src=0 if tabs[2] is None else tabs[2].shape[0], use_min_rank=min_rank is not None, min_rank=min_rank or 0,
+                               offset=offset, take=take if take >= 0 else np.iinfo(np.int64).max)
+        if cursor is not None:
+            sev, risk, label_gt, label_eq, id_gt = cursor
+            spec.has_cursor, spec.cur_sev, spec.cur_label_gt, spec.cur_label_eq, spec.cur_id_gt = 1, sev, label_gt, label_eq, id_gt
+            spec.cur_risk_null, spec.cur_risk = (1, 0.0) if risk is None else (0, risk)
+        lib = _lib.load()
+        res, total, selected, count = _vp(), C.c_int64(0), C.c_int64(0), C.c_int64(0)
+        with self._use() as h:
+            _lib.check(lib.abb_search_host(h, C.byref(spec), C.byref(res), C.byref(total), C.byref(selected), C.byref(count)))
+        try:
+            out = np.empty(count.value, np.int32)
+            _lib.check(lib.abb_search_fetch_host(res, out.ctypes.data))
+        finally:
+            lib.abb_search_result_free(res)
+        return out, int(total.value), int(selected.value)
+
     def betweenness(self) -> np.ndarray:
         """``nx.betweenness_centrality`` of the graph as a DiGraph (``abb_betweenness_host``): f64 per node."""
         out = np.zeros(self.n_nodes, dtype=np.float64)

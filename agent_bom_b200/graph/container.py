@@ -73,6 +73,7 @@ class UnifiedGraph:
         self._clusters = None              # semantic-cluster key table (graph/clusters.py)
         self._delta = None                 # snapshot-diff tables (graph/delta.py)
         self._lookup = None                # snapshot-lookup table and statistics (graph/lookup.py)
+        self._search = None                # node-search table (graph/search.py)
 
     # ── construction from foreign graphs ────────────────────────────────
     @classmethod
@@ -92,7 +93,7 @@ class UnifiedGraph:
     # ── mutation (reference container.py:116-198) ───────────────────────
     def _invalidate(self) -> None:
         self._csr = None
-        self._rank_inputs = self._focus_index = self._edge_lookup = self._clusters = self._delta = self._lookup = None
+        self._rank_inputs = self._focus_index = self._edge_lookup = self._clusters = self._delta = self._lookup = self._search = None
         if self._dg is not None:
             self._dg.close()
             self._dg = None

@@ -335,6 +335,64 @@ class B200GraphStore:
         g = self._snapshot(db, tenant_id, scan_id)
         return dict(EMPTY_STATS) if g is None else snapshot_stats(g)
 
+    def search_nodes(self, *, tenant_id: str = "", scan_id: str = "", query: str, entity_types: set[str] | None = None, min_severity_rank: int = 0,
+                     compliance_prefixes: set[str] | None = None, data_sources: set[str] | None = None, cursor: str | None = None, offset: int = 0,
+                     limit: int = 50) -> tuple[list, int, str | None]:
+        """``(nodes, total, next_cursor)`` of ``GET /v1/graph/search`` (reference api/graph_store.py:1346-1468): matched, filtered,
+        counted and paged on the device over the scan's search index (``scan_id or`` the latest scan); SQLite is asked only for the
+        page's records.  A bad cursor raises ``ValueError("Invalid graph cursor")``."""
+        db = self._sqlite_db()
+        if db is None:
+            return self._delegate("search_nodes", tenant_id=tenant_id, scan_id=scan_id, query=query, entity_types=entity_types,
+                                  min_severity_rank=min_severity_rank, compliance_prefixes=compliance_prefixes, data_sources=data_sources,
+                                  cursor=cursor, offset=offset, limit=limit)
+        from .graph.lookup import connect
+        from .graph.search import cursor_key, search_nodes
+        from .graph.snapshot import latest_snapshot_id
+
+        tenant = normalize_tenant(tenant_id)
+        if not scan_id:
+            conn = connect(db)
+            try:
+                scan_id = latest_snapshot_id(conn, tenant_id=tenant)
+            finally:
+                conn.close()
+            if not scan_id:
+                return [], 0, None
+        key = cursor_key(cursor)
+        g = self._graph(tenant, scan_id)
+        if g is None:
+            return [], 0, None
+        return search_nodes(g, db, tenant, query=query, entity_types=entity_types, min_severity_rank=min_severity_rank,
+                            compliance_prefixes=compliance_prefixes, data_sources=data_sources, key=key, offset=offset, limit=limit)
+
+    def page_nodes(self, *, tenant_id: str = "", scan_id: str = "", entity_types: set[str] | None = None, min_severity_rank: int = 0,
+                   cursor: str | None = None, offset: int = 0, limit: int = 500) -> tuple[str, str, list, int, str | None]:
+        """``(scan_id, created_at, nodes, total, next_cursor)`` of the snapshot's nodes in (severity, risk, label, id) order (reference
+        api/graph_store.py:1242-1313), filtered and paged on the device; ``GET /v1/graph/agents`` without ``q``."""
+        db = self._sqlite_db()
+        if db is None:
+            return self._delegate("page_nodes", tenant_id=tenant_id, scan_id=scan_id, entity_types=entity_types, min_severity_rank=min_severity_rank,
+                                  cursor=cursor, offset=offset, limit=limit)
+        from .graph.lookup import connect
+        from .graph.search import cursor_key, page_nodes
+        from .graph.snapshot import resolve_snapshot
+
+        tenant = normalize_tenant(tenant_id)
+        conn = connect(db)
+        try:
+            effective, created_at = resolve_snapshot(conn, tenant_id=tenant, scan_id=scan_id)
+        finally:
+            conn.close()
+        if not effective:
+            return scan_id, "", [], 0, None
+        key = cursor_key(cursor)
+        g = self._graph(tenant, effective)
+        if g is None:
+            return effective, created_at, [], 0, None
+        return (effective, created_at, *page_nodes(g, db, tenant, entity_types=entity_types, min_severity_rank=min_severity_rank, key=key,
+                                                   offset=offset, limit=limit))
+
     # ── everything else: the wrapped default store ──────────────────────
     def __getattr__(self, name: str):
         inner = self.__dict__.get("_inner")

@@ -546,6 +546,46 @@ int abb_lookup_context_host(abb_graph *g, int32_t node, abb_lookup_result **out,
 int abb_lookup_fetch_host(const abb_lookup_result *r, int32_t *edges_out);
 void abb_lookup_result_free(abb_lookup_result *r);
 
+/* ---- node search ----------------------------------------------------------------------------------------------
+ * Replace the per-request FTS5 MATCH / LIKE scan, COUNT(*) and sort of search_nodes and page_nodes
+ * (agent_bom/api/graph_store.py:1242-1313, 1346-1468).  The graph's search table (freed with the graph) is built in two calls:
+ * abb_search_text_host stores the stored search_text bytes of n nodes (text_off[n+1], int64; an empty row for a node without an
+ * index row) and sets, in cp_bits_out[0x110000 / 32], the bit of every code point >= 0x80 the text holds;
+ * abb_search_table_host folds the text into token text with fold[0x110000] (per code point: -1 separator, 0 folds away, else the
+ * code point it folds to; it must cover ASCII and every code point marked) and stores per node severity_id (INT32_MIN for NULL),
+ * risk (NaN for NULL), label rank, entity-type code (< n_types), compliance and data-source codes (< n_cmp / n_src, both -1 for a
+ * node without an index row).  Nodes are in id order: a node's index is its id rank.
+ * abb_search_host runs one call: mode 0 matches every node (page_nodes), mode 1 the nodes whose token text holds every pattern
+ * at a token start (FTS phrases: folded tokens joined by one space, none empty), mode 2 those whose raw text holds the one
+ * pattern (LIKE).  type_ok / cmp_ok / src_ok (NULL: off) are byte tables indexed by code; use_min_rank keeps severity_id >=
+ * min_rank.  *total_out counts the matches, *selected_out those that also pass the cursor (severity_id < cur_sev OR (= AND risk <
+ * cur_risk) OR (= AND = AND label rank >= cur_label_gt) OR (= AND = AND label rank == cur_label_eq AND node >= cur_id_gt), a
+ * NULL severity never passing and a NULL risk, or cur_risk_null, passing only through the first clause).  The page, positions
+ * [offset, offset + take) of the selection in (severity desc, risk desc, label, id) order with NULLs last, stays on the device
+ * in *out, owned by the caller; *count_out is its length and abb_search_fetch_host copies it.  All pointers are host memory. */
+typedef struct abb_search_spec {
+    int32_t mode, n_patterns;
+    const uint8_t *patterns;           /* pattern bytes */
+    const int64_t *pattern_off;        /* [n_patterns + 1] */
+    const uint8_t *type_ok, *cmp_ok, *src_ok;
+    int32_t n_types, n_cmp, n_src;     /* lengths of the tables given; must equal the search table's */
+    int32_t use_min_rank;
+    int64_t min_rank;
+    int32_t has_cursor, cur_risk_null;
+    int64_t cur_sev;
+    double cur_risk;
+    int64_t cur_label_gt, cur_label_eq, cur_id_gt;
+    int64_t offset, take;
+} abb_search_spec;
+int abb_search_text_host(abb_graph *g, int32_t n, const int64_t *text_off, const uint8_t *text, uint32_t *cp_bits_out);
+int abb_search_table_host(abb_graph *g, const int32_t *fold, const int32_t *severity, const double *risk, const uint32_t *label_rank,
+                          const int32_t *type_code, const int32_t *cmp_code, const int32_t *src_code, int32_t n_types, int32_t n_cmp, int32_t n_src);
+int64_t abb_search_table_bytes(const abb_graph *g);              /* device bytes of the search table, 0 when none */
+typedef struct abb_search_result abb_search_result;
+int abb_search_host(abb_graph *g, const abb_search_spec *spec, abb_search_result **out, int64_t *total_out, int64_t *selected_out, int64_t *count_out);
+int abb_search_fetch_host(const abb_search_result *r, int32_t *nodes_out);
+void abb_search_result_free(abb_search_result *r);
+
 #ifdef __cplusplus
 }
 #endif
