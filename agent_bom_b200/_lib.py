@@ -230,6 +230,9 @@ EXPORTS = {
     "abb_search_host": (C.c_int, [vp, vp, vp, vp, vp, vp]),
     "abb_search_fetch_host": (C.c_int, [vp, vp]),
     "abb_search_result_free": (None, [vp]),
+    "abb_compliance_table_host": (C.c_int, [vp, i32, vp, vp, vp, i32, vp, vp, i32, vp, i32, i32, i32, vp]),
+    "abb_compliance_table_bytes": (i64, [vp]),
+    "abb_compliance_fetch_host": (C.c_int, [vp, vp, vp, vp, vp, vp]),
 }
 
 _lock = threading.Lock()

@@ -36,6 +36,7 @@
 #include "walkb.cuh"
 #include "lookup.cuh"
 #include "search.cuh"
+#include "compliance.cuh"
 
 using namespace abb;
 
@@ -369,6 +370,13 @@ struct abb_graph {
     int64_t sr_n_long = 0;
     bool sr_ready = false;
     DevBuf sr_flags, sr_sel, sr_ctr, sr_pat, sr_tmp;
+    // compliance table (compliance_host.inl): (framework, severity), (framework, type) and (framework, tag) runs as [4][u] int64
+    // (framework, code, count, first row), node_count per framework and the first node ids per framework.  cm_sizes: the three run
+    // counts and the node-id count.  cm_ready = false until built.
+    DevBuf cm_sev, cm_type, cm_tag, cm_count, cm_rows;
+    int64_t cm_sizes[4] = {0, 0, 0, 0};
+    int32_t cm_nfw = 0;
+    bool cm_ready = false;
     // graph arrays of an uploaded graph (an adopted graph's belong to the caller)
     std::vector<DevBuf> owned_arrays;
 
@@ -1986,3 +1994,4 @@ extern "C" int abb_finding_context_host(abb_graph *g, int32_t max_depth, const i
 #include "delta_host.inl"
 #include "lookup_host.inl"
 #include "search_host.inl"
+#include "compliance_host.inl"

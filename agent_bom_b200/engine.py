@@ -695,6 +695,31 @@ class DeviceGraph:
         with self._use() as h:
             return int(_lib.load().abb_search_table_bytes(h))
 
+    def compliance_table(self, row_text, row_sev, row_type, text_off, text_tags, tag_fw, n_fw: int, n_sev: int, n_types: int) -> dict[str, np.ndarray]:
+        """Build the graph's compliance table (``abb_compliance_table_host``), replacing an earlier one, and return it
+        (``abb_compliance_fetch_host``): ``sev`` / ``type`` / ``tag`` runs [4, runs] int64 (framework, code, pairs, first row) in
+        (framework, code) order, ``node_count`` [n_fw] and ``node_rows``, the first 100 rows of each framework, frameworks in order.
+        Rows are in id order; ``text_off`` / ``text_tags``: the tag codes of each distinct text; ``tag_fw``: each tag's framework."""
+        row_text, row_sev, row_type, text_tags, tag_fw = (_i32(a) for a in (row_text, row_sev, row_type, text_tags, tag_fw))
+        text_off = np.ascontiguousarray(text_off, np.int64)
+        n = row_text.shape[0]
+        if row_sev.shape != (n,) or row_type.shape != (n,) or text_off.ndim != 1 or text_off.shape[0] < 1 or int(text_off[-1]) != text_tags.shape[0]:
+            raise ValueError("compliance table inputs have the wrong shapes")
+        sizes = np.zeros(4, np.int64)
+        lib = _lib.load()
+        with self._use() as h:
+            _lib.check(lib.abb_compliance_table_host(h, n, row_text.ctypes.data, row_sev.ctypes.data, row_type.ctypes.data, text_off.shape[0] - 1,
+                                                     text_off.ctypes.data, text_tags.ctypes.data, tag_fw.shape[0], tag_fw.ctypes.data, n_fw, n_sev,
+                                                     n_types, sizes.ctypes.data))
+            out = {"sev": np.empty((4, int(sizes[0])), np.int64), "type": np.empty((4, int(sizes[1])), np.int64),
+                   "tag": np.empty((4, int(sizes[2])), np.int64), "node_count": np.empty(n_fw, np.int64), "node_rows": np.empty(int(sizes[3]), np.int32)}
+            _lib.check(lib.abb_compliance_fetch_host(h, *(out[k].ctypes.data for k in ("sev", "type", "tag", "node_count", "node_rows"))))
+        return out
+
+    def compliance_table_bytes(self) -> int:
+        with self._use() as h:
+            return int(_lib.load().abb_compliance_table_bytes(h))
+
     def search(self, mode: int, patterns: list[bytes], type_ok=None, cmp_ok=None, src_ok=None, min_rank: int | None = None, cursor=None,
                offset: int = 0, take: int = -1) -> tuple[np.ndarray, int, int]:
         """One search or page call (``abb_search_host``): ``(page, total, selected)``, the page being node indices in page order.

@@ -74,6 +74,7 @@ class UnifiedGraph:
         self._delta = None                 # snapshot-diff tables (graph/delta.py)
         self._lookup = None                # snapshot-lookup table and statistics (graph/lookup.py)
         self._search = None                # node-search table (graph/search.py)
+        self._compliance = None            # compliance posture of the scan (graph/compliance.py)
 
     # ── construction from foreign graphs ────────────────────────────────
     @classmethod
@@ -93,7 +94,7 @@ class UnifiedGraph:
     # ── mutation (reference container.py:116-198) ───────────────────────
     def _invalidate(self) -> None:
         self._csr = None
-        self._rank_inputs = self._focus_index = self._edge_lookup = self._clusters = self._delta = self._lookup = self._search = None
+        self._rank_inputs = self._focus_index = self._edge_lookup = self._clusters = self._delta = self._lookup = self._search = self._compliance = None
         if self._dg is not None:
             self._dg.close()
             self._dg = None

@@ -393,6 +393,32 @@ class B200GraphStore:
         return (effective, created_at, *page_nodes(g, db, tenant, entity_types=entity_types, min_severity_rank=min_severity_rank, key=key,
                                                    offset=offset, limit=limit))
 
+    def compliance_summary(self, *, tenant_id: str = "", scan_id: str = "", framework: str = "") -> dict[str, Any]:
+        """The body of ``GET /v1/graph/compliance`` (reference api/graph_store.py:950-1031): per-framework finding counts, severity and
+        entity-type breakdowns, tags and member nodes of the snapshot (``scan_id or`` the latest), rolled up on the device once per
+        graph; ``framework`` selects one framework by its upper-cased prefix."""
+        db = self._sqlite_db()
+        if db is None:
+            return self._delegate("compliance_summary", tenant_id=tenant_id, scan_id=scan_id, framework=framework)
+        from .graph.compliance import compliance_summary, empty_summary
+        from .graph.lookup import connect
+        from .graph.snapshot import latest_snapshot_id
+
+        tenant = normalize_tenant(tenant_id)
+        effective = scan_id
+        if not effective:
+            conn = connect(db)
+            try:
+                effective = latest_snapshot_id(conn, tenant_id=tenant)
+            finally:
+                conn.close()
+            if not effective:
+                return empty_summary(scan_id)
+        g = self._graph(tenant, effective)
+        if g is None:
+            return empty_summary(effective)
+        return compliance_summary(g, db, tenant, framework)
+
     # ── everything else: the wrapped default store ──────────────────────
     def __getattr__(self, name: str):
         inner = self.__dict__.get("_inner")

@@ -586,6 +586,22 @@ int abb_search_host(abb_graph *g, const abb_search_spec *spec, abb_search_result
 int abb_search_fetch_host(const abb_search_result *r, int32_t *nodes_out);
 void abb_search_result_free(abb_search_result *r);
 
+/* ---- compliance posture ---------------------------------------------------------------------------------------
+ * Replace the per-request decode and Python loop over every (node, tag) pair of compliance_summary
+ * (agent_bom/api/graph_store.py:950-1031).  abb_compliance_table_host builds the graph's compliance table (freed with the graph,
+ * replacing an earlier one) from n tagged rows in id order: per row a text code (< n_texts), severity code (< n_sev) and
+ * entity-type code (< n_types); per text its tag codes text_tags[text_off[t] .. text_off[t+1]) (int64 offsets, repeats kept);
+ * per tag its framework code tag_fw[tag] (< n_fw).  Tags and frameworks are coded in the order their names sort.  It rolls up
+ * every (row, tag) pair and sets sizes_out[4]: the number of (framework, severity) runs, (framework, type) runs, distinct
+ * (framework, tag) pairs and node ids.  abb_compliance_fetch_host copies the table: each run array is [4][runs] int64 (framework,
+ * code, pairs, first row) in (framework, code) order; node_count[n_fw] the distinct rows per framework; node_rows the first 100
+ * of them per framework in row order, frameworks in order.  All pointers are host memory. */
+int abb_compliance_table_host(abb_graph *g, int32_t n, const int32_t *row_text, const int32_t *row_sev, const int32_t *row_type, int32_t n_texts,
+                              const int64_t *text_off, const int32_t *text_tags, int32_t n_tags, const int32_t *tag_fw, int32_t n_fw, int32_t n_sev,
+                              int32_t n_types, int64_t *sizes_out);
+int64_t abb_compliance_table_bytes(const abb_graph *g);          /* device bytes of the compliance table, 0 when none */
+int abb_compliance_fetch_host(abb_graph *g, int64_t *sev_runs, int64_t *type_runs, int64_t *tag_runs, int64_t *node_count, int32_t *node_rows);
+
 #ifdef __cplusplus
 }
 #endif
