@@ -204,6 +204,14 @@ EXPORTS = {
     "abb_lateral_result_width": (i32, [vp]),
     "abb_lateral_result_ms": (C.c_double, [vp]),
     "abb_lateral_result_free": (None, [vp]),
+    "abb_lateral_enrich_host": (C.c_int, [C.c_int, i32, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, i32, vp, vp, i64, i32, vp, C.POINTER(vp)]),
+    "abb_lateral_enrich_result_off": (vp, [vp]),
+    "abb_lateral_enrich_result_items": (vp, [vp]),
+    "abb_lateral_enrich_result_exec": (vp, [vp]),
+    "abb_lateral_enrich_result_severity": (vp, [vp]),
+    "abb_lateral_enrich_result_flags": (vp, [vp]),
+    "abb_lateral_enrich_result_ms": (C.c_double, [vp]),
+    "abb_lateral_enrich_result_free": (None, [vp]),
     "abb_group_union_host": (C.c_int, [C.c_int, i64, vp, vp, i64, vp, vp, vp, vp, C.POINTER(vp)]),
     "abb_union_result_off": (vp, [vp]),
     "abb_union_result_items": (vp, [vp]),

@@ -4,7 +4,7 @@ The reference keeps a second, older graph model next to ``UnifiedGraph``: ``Cont
 ``EdgeKind`` (``/root/reference/src/agent_bom/context_graph.py:54-130``).  Effective-reach scoring
 (``effective_reach.py``) is defined on that model, so the scorer here accepts any object of this shape — these
 records, or the reference's own ``build_context_graph`` output (duck-typed: ``nodes`` dict, ``edges`` list,
-``adjacency`` dict of per-node edge lists).  The scan-report → ContextGraph builder is out of scope (SURVEY §8).
+``adjacency`` dict of per-node edge lists).  ``context_report.build_context_graph`` builds these records from a scan report.
 """
 
 from __future__ import annotations

@@ -465,6 +465,32 @@ int32_t abb_lateral_result_width(const abb_lateral_result *r);           /* W = 
 double abb_lateral_result_ms(const abb_lateral_result *r);
 void abb_lateral_result_free(abb_lateral_result *r);
 
+/* Enrichment of found lateral paths: what _build_lateral_path (agent_bom/context_graph.py:495-572) folds into each path,
+ * computed for many paths at once.  Per path: the kept labels in first-add order, each category << 30 | label id (category 0
+ * credential, 1 tool, 2 vulnerability; a credential name carried by a shares_credential link shares the credential ids), the
+ * number of execute-capable tools and the highest severity score among first-added labels.
+ * adj_* as for abb_lateral_paths_host; adj_name: per entry, for shares_server_kind entries the surface of the link's server
+ * name, for shares_credential_kind entries the credential id of the link's credential name, -1 when the name is empty or absent.
+ * node_label: label id of credential / tool / vulnerability nodes (< 2^30); node_value: tools 1 execute / 0 not, vulnerabilities
+ * their severity score, -1 when the node's test raised; node_surface: a server node's surface, -1 when it has none.
+ * surface_off[n_surfaces+1] / surface_node: per surface the credential / tool / vulnerability nodes that first add each label of
+ * it, in order (each server's exposes / provides / vulnerable_to entries, and per shared server name those of every server with
+ * that label in node order).  records: [n_paths][width+2] as abb_lateral_result_records gives them.
+ * flags bit0: a first-added label's value is -1 (the caller re-derives that path to raise what the reference raises). */
+typedef struct abb_lateral_enrich_result abb_lateral_enrich_result;
+int abb_lateral_enrich_host(int device, int32_t n_nodes, const int64_t *adj_off, const int32_t *adj_nbr, const uint8_t *adj_kind,
+                            const int32_t *adj_name, int32_t shares_server_kind, int32_t shares_credential_kind, const uint8_t *node_kind,
+                            const int32_t *node_label, const float *node_value, const int32_t *node_surface, int32_t n_surfaces,
+                            const int64_t *surface_off, const int32_t *surface_node, int64_t n_paths, int32_t width, const int32_t *records,
+                            abb_lateral_enrich_result **out);
+const int64_t *abb_lateral_enrich_result_off(const abb_lateral_enrich_result *r);     /* [n_paths+1] */
+const int32_t *abb_lateral_enrich_result_items(const abb_lateral_enrich_result *r);   /* [off[n_paths]] */
+const int32_t *abb_lateral_enrich_result_exec(const abb_lateral_enrich_result *r);    /* [n_paths] */
+const float *abb_lateral_enrich_result_severity(const abb_lateral_enrich_result *r);  /* [n_paths] */
+const int32_t *abb_lateral_enrich_result_flags(const abb_lateral_enrich_result *r);   /* [n_paths] */
+double abb_lateral_enrich_result_ms(const abb_lateral_enrich_result *r);
+void abb_lateral_enrich_result_free(abb_lateral_enrich_result *r);
+
 /* ---- per-group union of member item lists (effective-reach scoring) ------------------------------------------
  * Replaces the per-vulnerability reduction of agent_bom/effective_reach.py:372-426 (`compute`): for every group
  * (a vulnerability) over its members (the servers VULNERABLE_TO it, effective_reach.py:265-279) return
