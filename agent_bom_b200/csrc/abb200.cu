@@ -184,6 +184,20 @@ static int cub_run(DevBuf &tmp, F &&call) {
     return ABB_OK;
 }
 
+// One kernel launch: enqueues `kern` with this configuration on `st`, counts it, and fails with ABB_ERR_CUDA under the caller's file and
+// line when the launch is refused (bad configuration, too much shared memory, no image for the device).  The arguments convert to the
+// kernel's parameter types as in a direct launch.  Call it as LAUNCH(kernel, grid, block, smem, stream, args...): C++17 has no
+// std::source_location, so the macro supplies the call site.
+template <class... P, class... A>
+static int launch_at(const char *file, int line, void (*kern)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, A &&...args) {
+    kern<<<grid, block, smem, st>>>(std::forward<A>(args)...);
+    g_launches++;
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(ABB_ERR_CUDA, "kernel launch failed: %s (%s:%d)", cudaGetErrorString(e), file, line);
+    return ABB_OK;
+}
+#define LAUNCH(...) launch_at(__FILE__, __LINE__, __VA_ARGS__)
+
 // exclusive prefix sum of n int64 values; `sync` waits for it
 static int scan_i64(DevBuf &tmp, const int64_t *in, int64_t *out, int64_t n, cudaStream_t st, bool sync = false) {
     if (int rc = cub_run(tmp, [&](void *t, size_t &b) { return cub::DeviceScan::ExclusiveSum(t, b, in, out, static_cast<int>(n), st); })) return rc;
@@ -664,10 +678,7 @@ static int launch_smem(const abb_graph *g, const WalkArgs &A, int64_t max_items,
     int64_t grid = static_cast<int64_t>(g->sm_count) * occ_cache;
     int64_t need = (max_items + static_cast<int64_t>(WARPS) * WORK_CHUNK - 1) / (static_cast<int64_t>(WARPS) * WORK_CHUNK);
     grid = std::max<int64_t>(1, std::min(grid, need));
-    kern<<<static_cast<unsigned>(grid), WARPS * 32, smem, st>>>(A);
-    g_launches++;
-    CUDA_TRY(cudaGetLastError());
-    return ABB_OK;
+    return LAUNCH(kern, static_cast<unsigned>(grid), WARPS * 32, smem, st, A);
 }
 
 template <int H, int Q, int WARPS>
@@ -683,18 +694,17 @@ static int launch_smem_variant(const abb_graph *g, const WalkArgs &A, int64_t ma
 static int launch_global_variant(const WalkArgs &A, int slots, int sm_count, bool meta, bool bud, cudaStream_t st) {
     const int blocks = std::max(1, slots / 4);
     const bool dense = slots > sm_count * 40;      // more than 40 warps per SM: the 40-register build (12 blocks of 4 warps per SM)
+    void (*kern)(WalkArgs);
     if (dense) {
-        if (meta && bud) walk_global_kernel<true, true, 12><<<blocks, 128, 0, st>>>(A);
-        else if (meta) walk_global_kernel<true, false, 12><<<blocks, 128, 0, st>>>(A);
-        else if (bud) walk_global_kernel<false, true, 12><<<blocks, 128, 0, st>>>(A);
-        else walk_global_kernel<false, false, 12><<<blocks, 128, 0, st>>>(A);
-    } else if (meta && bud) walk_global_kernel<true, true, 10><<<blocks, 128, 0, st>>>(A);
-    else if (meta) walk_global_kernel<true, false, 10><<<blocks, 128, 0, st>>>(A);
-    else if (bud) walk_global_kernel<false, true, 10><<<blocks, 128, 0, st>>>(A);
-    else walk_global_kernel<false, false, 10><<<blocks, 128, 0, st>>>(A);
-    g_launches++;
-    CUDA_TRY(cudaGetLastError());
-    return ABB_OK;
+        if (meta && bud) kern = walk_global_kernel<true, true, 12>;
+        else if (meta) kern = walk_global_kernel<true, false, 12>;
+        else if (bud) kern = walk_global_kernel<false, true, 12>;
+        else kern = walk_global_kernel<false, false, 12>;
+    } else if (meta && bud) kern = walk_global_kernel<true, true, 10>;
+    else if (meta) kern = walk_global_kernel<true, false, 10>;
+    else if (bud) kern = walk_global_kernel<false, true, 10>;
+    else kern = walk_global_kernel<false, false, 10>;
+    return LAUNCH(kern, blocks, 128, 0, st, A);
 }
 
 template <int W, bool QSM, bool PAR, bool META, int MINB>
@@ -713,10 +723,7 @@ static int launch_block(const abb_graph *g, const WalkArgs &A, const BlockTier &
     }
     int grid = g->sm_count * occ_cache;
     if (grid_cap > 0) grid = std::min(grid, grid_cap);
-    kern<<<static_cast<unsigned>(grid), W * 32, smem, st>>>(A, T);
-    g_launches++;
-    CUDA_TRY(cudaGetLastError());
-    return ABB_OK;
+    return LAUNCH(kern, static_cast<unsigned>(grid), W * 32, smem, st, A, T);
 }
 
 // Up to five tiers on one stream.  `A` carries spec/io and the first tier's work list (qlist/nq/nq_dev); every later
@@ -749,8 +756,7 @@ static int enqueue_tiers(abb_graph *g, WalkArgs A, int64_t max_items, unsigned l
     bool front_taken = false;                       // S1's heavy part routed (to the big tier when few, else first in line for the warp tier)
     unsigned long long *to_big = ctl + CTL_ROUTE, *to_warp = ctl + CTL_ROUTE + 1;
     if (plain && (g->block_tiers & 2) && idb <= 26) {
-        route_heavy_kernel<<<1, 1, 0, st>>>(ctl + 1, to_big, to_warp, static_cast<unsigned long long>(g->big_limit));
-        g_launches++;
+        if (int rc = LAUNCH(route_heavy_kernel, 1, 1, 0, st, ctl + 1, to_big, to_warp, static_cast<unsigned long long>(g->big_limit))) return rc;
         // big tier: the heavy (front) part of S1's list; what it cannot hold goes to a list of its own (ovs[2]) that the next tier
         // reads after S1's back part — NOT onto S1's list: front + back may already fill it
         A.qlist = ovs[0]; A.nq = 0; A.nq_dev = to_big; A.nq_back_dev = nullptr; A.ctl = ctl + 4 * 1;
@@ -841,20 +847,20 @@ static int enqueue_dedup_walk(abb_graph *g, const abb_walk_spec *spec, const abb
     const unsigned blocks = static_cast<unsigned>((nq + 255) / 256);
     CUDA_TRY(cudaMemsetAsync(cnt, 0, 8 * sizeof(unsigned long long), st));
     CUDA_TRY(cudaMemsetAsync(glen, 0, q1 * 8, st));
-    dedup_sig_kernel<<<blocks, 256, 0, st>>>(g->v, *spec, io->roots, nq, sig, qi); g_launches++;
+    if ((rc = LAUNCH(dedup_sig_kernel, blocks, 256, 0, st, g->v, *spec, io->roots, nq, sig, qi))) return rc;
     if ((rc = cub_run(g->dd_tmp, [&](void *t, size_t &b) { return cub::DeviceRadixSort::SortPairs(t, b, sig, ssig, qi, sq, static_cast<int>(nq), 0, SIG_BITS, st); })))
         return rc;
-    dedup_heads_kernel<<<blocks, 256, 0, st>>>(ssig, sq, nq, head, indiv, cnt); g_launches++;
+    if ((rc = LAUNCH(dedup_heads_kernel, blocks, 256, 0, st, ssig, sq, nq, head, indiv, cnt))) return rc;
     cub::TransformInputIterator<int64_t, HeadToI64, const uint8_t *> head64(head, HeadToI64());
     if ((rc = cub_run(g->dd_tmp, [&](void *t, size_t &b) { return cub::DeviceScan::InclusiveSum(t, b, head64, gid, static_cast<int>(nq), st); }))) return rc;
     if ((rc = select_flagged(g->dd_tmp, head, hp, cnt, static_cast<int>(nq), st))) return rc;
-    dedup_groups_kernel<<<static_cast<unsigned>((nq + 1 + 255) / 256), 256, 0, st>>>(g->v, *spec, io->roots, sq, hp, cnt, glen, memoff); g_launches++;
+    if ((rc = LAUNCH(dedup_groups_kernel, static_cast<unsigned>((nq + 1 + 255) / 256), 256, 0, st, g->v, *spec, io->roots, sq, hp, cnt, glen, memoff))) return rc;
     // glen is passed non-const here, unlike scan_i64's input: a different cub instantiation
     if ((rc = cub_run(g->dd_tmp, [&](void *t, size_t &b) { return cub::DeviceScan::ExclusiveSum(t, b, glen, goff, static_cast<int>(nq + 1), st); }))) return rc;
-    dedup_roots_kernel<<<blocks, 256, 0, st>>>(g->v, *spec, io->roots, sq, hp, cnt, goff, g->dd_arena.as<int32_t>()); g_launches++;
-    dedup_members_kernel<<<blocks, 256, 0, st>>>(g->v, *spec, io->roots, sq, head, gid, goff, g->dd_arena.as<int32_t>(), g->dd_memsrc.as<int32_t>(),
-                                                  g->dd_memstate.as<int32_t>(), indiv, cnt); g_launches++;
-    CUDA_TRY(cudaGetLastError());
+    if ((rc = LAUNCH(dedup_roots_kernel, blocks, 256, 0, st, g->v, *spec, io->roots, sq, hp, cnt, goff, g->dd_arena.as<int32_t>()))) return rc;
+    if ((rc = LAUNCH(dedup_members_kernel, blocks, 256, 0, st, g->v, *spec, io->roots, sq, head, gid, goff, g->dd_arena.as<int32_t>(), g->dd_memsrc.as<int32_t>(),
+                     g->dd_memstate.as<int32_t>(), indiv, cnt)))
+        return rc;
     unsigned long long *ctl = g->ctl.as<unsigned long long>();
     // canonical walks: one per group, seeded with the shared frontier, one level shallower, depths biased by one
     WalkArgs C{};
@@ -869,7 +875,7 @@ static int enqueue_dedup_walk(abb_graph *g, const abb_walk_spec *spec, const abb
         // walk order = first-seed order (a 2 M-key radix sort over the node-id bits, ~0.1 ms): neighbouring groups share rows in L2
         uint32_t *lkey = g->dd_lkey.as<uint32_t>(), *lkey2 = g->dd_lkey2.as<uint32_t>();
         int32_t *lgid = g->dd_lgid.as<int32_t>(), *order = g->dd_order.as<int32_t>();
-        dedup_locality_keys_kernel<<<blocks, 256, 0, st>>>(cnt, goff, g->dd_arena.as<int32_t>(), lkey, lgid, nq); g_launches++;
+        if ((rc = LAUNCH(dedup_locality_keys_kernel, blocks, 256, 0, st, cnt, goff, g->dd_arena.as<int32_t>(), lkey, lgid, nq))) return rc;
         if ((rc = cub_run(g->dd_tmp, [&](void *t, size_t &b) { return cub::DeviceRadixSort::SortPairs(t, b, lkey, lkey2, lgid, order, static_cast<int>(nq), 0, 32, st); })))
             return rc;
         C.qlist = order;
@@ -877,11 +883,10 @@ static int enqueue_dedup_walk(abb_graph *g, const abb_walk_spec *spec, const abb
     C.depth_bias = 1; C.hist_roots = 1;
     C.mem_off = memoff; C.mem_src = g->dd_memsrc.as<int32_t>(); C.mem_state = g->dd_memstate.as<int32_t>();
     if ((rc = enqueue_tiers(g, C, nq, ctl, st))) return rc;
-    dedup_share_kernel<<<grid_for(nq, 256, g->sm_count, 8), 256, 0, st>>>(
-        sq, gid, g->dd_memstate.as<int32_t>(), cnt, C.io.q_start, C.io.q_count, C.io.q_maxd, C.io.q_flags, C.io.q_hist, io->q_start, io->q_count, io->q_maxd,
-        io->q_flags, (fl & ABB_WALK_HIST) ? io->q_hist : nullptr, indiv, cnt);
-    g_launches++;
-    CUDA_TRY(cudaGetLastError());
+    if ((rc = LAUNCH(dedup_share_kernel, grid_for(nq, 256, g->sm_count, 8), 256, 0, st,
+                     sq, gid, g->dd_memstate.as<int32_t>(), cnt, C.io.q_start, C.io.q_count, C.io.q_maxd, C.io.q_flags, C.io.q_hist, io->q_start, io->q_count,
+                     io->q_maxd, io->q_flags, (fl & ABB_WALK_HIST) ? io->q_hist : nullptr, indiv, cnt)))
+        return rc;
     // individual walks: ineligible sources, signature collisions, sources reached by their own group's walk
     WalkArgs I{};
     I.g = g->v; I.spec = *spec; I.io = *io;
@@ -931,10 +936,7 @@ extern "C" int abb_walk_signatures(abb_graph *g, const abb_walk_spec *spec, cons
     if (!g || !spec || n < 0 || (n && (!roots || !sig))) return fail(ABB_ERR_ARG, "bad arguments");
     if (!n) return ABB_OK;
     DeviceGuard dg(g->device);
-    dedup_sig_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(g->v, *spec, roots, n, sig, nullptr);
-    g_launches++;
-    CUDA_TRY(cudaGetLastError());
-    return ABB_OK;
+    return LAUNCH(dedup_sig_kernel, static_cast<unsigned>((n + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream), g->v, *spec, roots, n, sig, nullptr);
 }
 
 extern "C" float abb_last_walk_ms(abb_graph *g) {
@@ -1067,8 +1069,9 @@ static int check_tier_fatal(abb_graph *g) {
 static int scan_hist_columns(abb_graph *g, const uint32_t *q_hist, int64_t nq, cudaStream_t st) {
     if (int rc = g->d_histinfo.ensure(2 * sizeof(unsigned long long))) return rc;
     CUDA_TRY(cudaMemsetAsync(g->d_histinfo.p, 0, 2 * sizeof(unsigned long long), st));
-    hist_columns_kernel<<<static_cast<unsigned>(g->sm_count) * 8, 256, 0, st>>>(q_hist, nq * ABB_N_ENTITY_TYPES, g->d_histinfo.as<unsigned long long>());
-    g_launches++;
+    if (int rc = LAUNCH(hist_columns_kernel, static_cast<unsigned>(g->sm_count) * 8, 256, 0, st, q_hist, nq * ABB_N_ENTITY_TYPES,
+                        g->d_histinfo.as<unsigned long long>()))
+        return rc;
     CUDA_TRY(cudaMemcpyAsync(g->hist_info, g->d_histinfo.p, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
     return ABB_OK;
 }
@@ -1215,9 +1218,9 @@ static int walk_collect(abb_graph *g, const abb_walk_spec *spec, const abb_walk_
             const size_t pbytes = q * hc.k * r->hist_width;
             if (int rc = g->d_hist_packed.ensure(pbytes)) return rc;
             const unsigned grid = static_cast<unsigned>(g->sm_count) * 8;
-            if (r->hist_width == 2) hist_pack_kernel<uint16_t><<<grid, 256, 0, st>>>(io.q_hist, nq, hc, g->d_hist_packed.as<uint16_t>());
-            else hist_pack_kernel<uint32_t><<<grid, 256, 0, st>>>(io.q_hist, nq, hc, g->d_hist_packed.as<uint32_t>());
-            g_launches++;
+            const int rc = r->hist_width == 2 ? LAUNCH(hist_pack_kernel<uint16_t>, grid, 256, 0, st, io.q_hist, nq, hc, g->d_hist_packed.as<uint16_t>())
+                                              : LAUNCH(hist_pack_kernel<uint32_t>, grid, 256, 0, st, io.q_hist, nq, hc, g->d_hist_packed.as<uint32_t>());
+            if (rc) return rc;
             d2h.keep(cudaGetLastError());
             d2h(r->q_hist_packed, g->d_hist_packed.p, pbytes);
         }
@@ -1283,16 +1286,18 @@ static int walk_host_chunked(abb_graph *g, const abb_walk_spec *spec, const int3
     unsigned long long *sig = nullptr;
     if (by_sig) {
         sig = g->ck_sig.as<unsigned long long>();
-        dedup_sig_kernel<<<qblocks, 256, 0, st>>>(g->v, *spec, g->d_roots.as<int32_t>(), nq, sig, nullptr); g_launches++;
+        if ((rc = LAUNCH(dedup_sig_kernel, qblocks, 256, 0, st, g->v, *spec, g->d_roots.as<int32_t>(), nq, sig, nullptr))) { drain(); return rc; }
     }
     CUDA_TRY(cudaMemsetAsync(g->ck_counts.p, 0, 64 * 8, st));
-    chunk_key_kernel<<<qblocks, 256, 0, st>>>(sig, nq, K, g->ck_key.as<uint32_t>(), g->ck_idx.as<int32_t>(), g->ck_counts.as<unsigned long long>()); g_launches++;
+    if ((rc = LAUNCH(chunk_key_kernel, qblocks, 256, 0, st, sig, nq, K, g->ck_key.as<uint32_t>(), g->ck_idx.as<int32_t>(), g->ck_counts.as<unsigned long long>()))) {
+        drain(); return rc;
+    }
     if ((rc = cub_run(g->ck_tmp, [&](void *t, size_t &b) {
              return cub::DeviceRadixSort::SortPairs(t, b, g->ck_key.as<uint32_t>(), g->ck_key2.as<uint32_t>(), g->ck_idx.as<int32_t>(), g->ck_order.as<int32_t>(),
                                                     static_cast<int>(nq), 0, 6, st);
          }))) { drain(); return rc; }
     const int32_t *order = g->ck_order.as<int32_t>();      // order[i] = caller index of the i-th query in chunk order
-    gather_i32_kernel<<<qblocks, 256, 0, st>>>(g->d_roots.as<int32_t>(), order, g->ck_roots.as<int32_t>(), nq); g_launches++;
+    if ((rc = LAUNCH(gather_i32_kernel, qblocks, 256, 0, st, g->d_roots.as<int32_t>(), order, g->ck_roots.as<int32_t>(), nq))) { drain(); return rc; }
     unsigned long long counts[64] = {0};
     CUDA_TRY(cudaMemcpyAsync(counts, g->ck_counts.p, 64 * 8, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
@@ -1334,7 +1339,8 @@ static int walk_host_chunked(abb_graph *g, const abb_walk_spec *spec, const int3
             g->chunk_hint_nq = -1;
             return ABB_RETRY_UNCHUNKED;
         }
-        if (node_base) { add_base_kernel<<<static_cast<unsigned>((nk + 255) / 256), 256, 0, st>>>(g->d_qstart.as<int64_t>() + b0, nk, node_base); g_launches++; }
+        if (node_base)
+            if ((rc = LAUNCH(add_base_kernel, static_cast<unsigned>((nk + 255) / 256), 256, 0, st, g->d_qstart.as<int64_t>() + b0, nk, node_base))) { drain(); return rc; }
         CUDA_TRY(cudaEventRecord(g->ev_chunk_walked, st));
         CUDA_TRY(cudaStreamWaitEvent(cst, g->ev_chunk_walked, 0));
         if (tot) CUDA_TRY(cudaMemcpyAsync(r->nodes.as<int32_t>() + node_base, arena.p, static_cast<size_t>(tot) * 4, cudaMemcpyDeviceToHost, cst));
@@ -1350,11 +1356,12 @@ static int walk_host_chunked(abb_graph *g, const abb_walk_spec *spec, const int3
     r->d2h += node_base * 4;
     // per-query results back into caller order, then to the host (the node copies of the last chunks are still in flight on the copy stream)
     const unsigned sgrid = static_cast<unsigned>(g->sm_count) * 8;
-    scatter_rows_kernel<int64_t><<<sgrid, 256, 0, st>>>(g->d_qstart.as<int64_t>(), order, g->ck_qstart.as<int64_t>(), nq, 1);
-    scatter_rows_kernel<int32_t><<<sgrid, 256, 0, st>>>(g->d_qcount.as<int32_t>(), order, g->ck_qcount.as<int32_t>(), nq, 1);
-    scatter_rows_kernel<int32_t><<<sgrid, 256, 0, st>>>(g->d_qmaxd.as<int32_t>(), order, g->ck_qmaxd.as<int32_t>(), nq, 1);
-    scatter_rows_kernel<int32_t><<<sgrid, 256, 0, st>>>(g->d_qflags.as<int32_t>(), order, g->ck_qflags.as<int32_t>(), nq, 1);
-    g_launches += 4;
+    if ((rc = LAUNCH(scatter_rows_kernel<int64_t>, sgrid, 256, 0, st, g->d_qstart.as<int64_t>(), order, g->ck_qstart.as<int64_t>(), nq, 1)) ||
+        (rc = LAUNCH(scatter_rows_kernel<int32_t>, sgrid, 256, 0, st, g->d_qcount.as<int32_t>(), order, g->ck_qcount.as<int32_t>(), nq, 1)) ||
+        (rc = LAUNCH(scatter_rows_kernel<int32_t>, sgrid, 256, 0, st, g->d_qmaxd.as<int32_t>(), order, g->ck_qmaxd.as<int32_t>(), nq, 1)) ||
+        (rc = LAUNCH(scatter_rows_kernel<int32_t>, sgrid, 256, 0, st, g->d_qflags.as<int32_t>(), order, g->ck_qflags.as<int32_t>(), nq, 1))) {
+        drain(); return rc;
+    }
     const bool scan_hist = hist && g->hist_pack && nq >= 1024;
     if (scan_hist) {
         if ((rc = scan_hist_columns(g, g->d_qhist.as<uint32_t>(), nq, st))) { drain(); return rc; }
@@ -1368,16 +1375,18 @@ static int walk_host_chunked(abb_graph *g, const abb_walk_spec *spec, const int3
             const size_t pbytes = q * hc.k * r->hist_width;
             if (!r->q_hist_packed.alloc(pbytes)) { drain(); return fail(ABB_ERR_NOMEM, "pinned host allocation failed"); }
             if ((rc = g->d_hist_packed.ensure(pbytes))) { drain(); return rc; }
-            if (r->hist_width == 2) hist_pack_scatter_kernel<uint16_t><<<sgrid, 256, 0, st>>>(g->d_qhist.as<uint32_t>(), order, nq, hc, g->d_hist_packed.as<uint16_t>());
-            else hist_pack_scatter_kernel<uint32_t><<<sgrid, 256, 0, st>>>(g->d_qhist.as<uint32_t>(), order, nq, hc, g->d_hist_packed.as<uint32_t>());
-            g_launches++;
+            rc = r->hist_width == 2
+                     ? LAUNCH(hist_pack_scatter_kernel<uint16_t>, sgrid, 256, 0, st, g->d_qhist.as<uint32_t>(), order, nq, hc, g->d_hist_packed.as<uint16_t>())
+                     : LAUNCH(hist_pack_scatter_kernel<uint32_t>, sgrid, 256, 0, st, g->d_qhist.as<uint32_t>(), order, nq, hc, g->d_hist_packed.as<uint32_t>());
+            if (rc) { drain(); return rc; }
             d2h(r->q_hist_packed, g->d_hist_packed.p, pbytes);
         }
     } else if (hist) {
         if (!r->q_hist.alloc(q * ABB_N_ENTITY_TYPES * 4)) { drain(); return fail(ABB_ERR_NOMEM, "pinned host allocation failed"); }
         if ((rc = g->ck_qhist.ensure(q1 * ABB_N_ENTITY_TYPES * 4))) { drain(); return rc; }
-        scatter_rows_kernel<uint32_t><<<sgrid, 256, 0, st>>>(g->d_qhist.as<uint32_t>(), order, g->ck_qhist.as<uint32_t>(), nq, ABB_N_ENTITY_TYPES);
-        g_launches++;
+        if ((rc = LAUNCH(scatter_rows_kernel<uint32_t>, sgrid, 256, 0, st, g->d_qhist.as<uint32_t>(), order, g->ck_qhist.as<uint32_t>(), nq, ABB_N_ENTITY_TYPES))) {
+            drain(); return rc;
+        }
         d2h(r->q_hist, g->ck_qhist.p, q * ABB_N_ENTITY_TYPES * 4);
     }
     cudaError_t &e = d2h.err;
@@ -1418,23 +1427,22 @@ static int ensure_server_table(abb_graph *g, cudaStream_t st) {
     if (int rc = g->srv_cred.ensure(n * 4)) return rc;
     if (int rc = g->srv_tool.ensure(n * 4)) return rc;
     const unsigned grid = grid_for(g->v.n, 256, g->sm_count, 16);
-    server_table_kernel<<<grid, 256, 0, st>>>(g->v, g->srv_cred.as<int32_t>(), g->srv_tool.as<int32_t>());
-    g_launches++;
+    if (int rc = LAUNCH(server_table_kernel, grid, 256, 0, st, g->v, g->srv_cred.as<int32_t>(), g->srv_tool.as<int32_t>())) return rc;
     // principal rows of every server (paths.cuh server_rows_kernel): count, scan in place, fill
     if (int rc = g->srv_roff.ensure(n * 8)) return rc;
     int64_t *roff = g->srv_roff.as<int64_t>();
     CUDA_TRY(cudaMemsetAsync(roff, 0, n * 8, st));
-    server_rows_kernel<false><<<grid, 256, 0, st>>>(g->v, g->srv_cred.as<int32_t>(), g->srv_tool.as<int32_t>(), roff, nullptr, nullptr);
-    g_launches++;
+    if (int rc = LAUNCH(server_rows_kernel<false>, grid, 256, 0, st, g->v, g->srv_cred.as<int32_t>(), g->srv_tool.as<int32_t>(), roff, nullptr, nullptr))
+        return rc;
     if (int rc = scan_i64(g->p_scan_tmp, roff, roff, static_cast<int64_t>(n), st)) return rc;
     int64_t total = 0;
     CUDA_TRY(cudaMemcpyAsync(&total, roff + g->v.n, 8, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     if (int rc = g->srv_row.ensure(static_cast<size_t>(total + 1) * 16)) return rc;
     if (int rc = g->srv_rel.ensure(static_cast<size_t>(total) + 16)) return rc;
-    server_rows_kernel<true><<<grid, 256, 0, st>>>(g->v, g->srv_cred.as<int32_t>(), g->srv_tool.as<int32_t>(), roff, g->srv_row.as<int4>(), g->srv_rel.as<int8_t>());
-    g_launches++;
-    CUDA_TRY(cudaGetLastError());
+    if (int rc = LAUNCH(server_rows_kernel<true>, grid, 256, 0, st, g->v, g->srv_cred.as<int32_t>(), g->srv_tool.as<int32_t>(), roff, g->srv_row.as<int4>(),
+                        g->srv_rel.as<int8_t>()))
+        return rc;
     CUDA_TRY(cudaStreamSynchronize(st));   // one-time: later launches may come on other streams
     g->srv_table_ready = true;
     return ABB_OK;
@@ -1489,9 +1497,9 @@ static int ensure_exposure_tables(abb_graph *g, cudaStream_t st) {
     CUDA_TRY(cudaMemsetAsync(A.x_toff, 0, n1 * 8, st));
     CUDA_TRY(cudaMemsetAsync(A.x_overflow, 0, 4, st));
     const unsigned grid = warp_grid(g, (n + 31) / 32);
-    node_links_kernel<false><<<grid, 256, 0, st>>>(A); g_launches++;
+    if ((rc = LAUNCH(node_links_kernel<false>, grid, 256, 0, st, A))) return rc;
     if ((rc = scan_i64(g->p_scan_tmp, A.x_loff, A.x_loff, n + 1, st))) return rc;
-    template_kernel<false><<<grid, 256, 0, st>>>(A); g_launches++;
+    if ((rc = LAUNCH(template_kernel<false>, grid, 256, 0, st, A))) return rc;
     if ((rc = scan_i64(g->p_scan_tmp, A.x_toff, A.x_toff, n + 1, st))) return rc;
     int64_t NL = 0, TR = 0;
     CUDA_TRY(cudaMemcpyAsync(&NL, A.x_loff + n, 8, cudaMemcpyDeviceToHost, st));
@@ -1504,10 +1512,8 @@ static int ensure_exposure_tables(abb_graph *g, cudaStream_t st) {
     if (!rc) rc = g->x_trel.alloc(static_cast<size_t>(TR) * 2);
     if (rc) return rc;
     A = paths_base(g);
-    template_kernel<true><<<grid, 256, 0, st>>>(A); g_launches++;
-    node_links_kernel<true><<<grid, 256, 0, st>>>(A); g_launches++;
+    if ((rc = LAUNCH(template_kernel<true>, grid, 256, 0, st, A)) || (rc = LAUNCH(node_links_kernel<true>, grid, 256, 0, st, A))) return rc;
     unsigned overflow = 0;
-    CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaMemcpyAsync(&overflow, A.x_overflow, 4, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     if (overflow) return fail(ABB_ERR_CAPACITY, "exposure tables: a finding has 2^31 or more exposure-path rows");
@@ -1531,9 +1537,8 @@ static int enqueue_paths_count(abb_graph *g, const abb_paths_io *io, cudaStream_
     if (rc) return rc;
     PathsArgs A = paths_base(g);
     A.io = *io; A.f_cnt = g->pl_cnt.as<int64_t>(); A.f_link = g->pl_link.as<int2>(); A.f_lcnt = link_counts ? g->pl_lcnt.as<int64_t>() : nullptr;
-    finding_rows_kernel<<<static_cast<unsigned>((nf + 1 + 255) / 256), 256, 0, st>>>(A); g_launches++;
+    if ((rc = LAUNCH(finding_rows_kernel, static_cast<unsigned>((nf + 1 + 255) / 256), 256, 0, st, A))) return rc;
     if ((rc = scan_i64(g->p_scan_tmp, A.f_cnt, io->f_off, nf + 1, st))) return rc;
-    CUDA_TRY(cudaGetLastError());
     g->paths_args = A;
     g->paths_args_valid = true;
     return ABB_OK;
@@ -1547,10 +1552,7 @@ static int enqueue_paths_fill(abb_graph *g, const abb_paths_io *io, cudaStream_t
     if ((reinterpret_cast<uintptr_t>(io->hops) & 15) != 0 || (reinterpret_cast<uintptr_t>(io->rels) & 3) != 0) return fail(ABB_ERR_ARG, "io.hops must be 16-byte and io.rels 4-byte aligned");
     PathsArgs A = g->paths_args;
     A.io = *io;
-    replicate_kernel<<<row_grid(g, replicate_kernel, g->replicate_grid), ROW_THREADS, 0, st>>>(A);
-    g_launches++;
-    CUDA_TRY(cudaGetLastError());
-    return ABB_OK;
+    return LAUNCH(replicate_kernel, row_grid(g, replicate_kernel, g->replicate_grid), ROW_THREADS, 0, st, A);
 }
 
 extern "C" int abb_paths_count_launch(abb_graph *g, const abb_paths_io *io, void *stream) {
@@ -1683,10 +1685,10 @@ static int paths_run(abb_graph *g, const int32_t *h_findings, const int32_t *d_f
     uint8_t *need = g->pl_need.as<uint8_t>();
     unsigned long long *nu = g->pl_nu.as<unsigned long long>();
     CUDA_TRY(cudaMemsetAsync(need, 0, static_cast<size_t>(n) + 16, st));
-    batch_links_kernel<<<static_cast<unsigned>((nf + 1 + 255) / 256), 256, 0, st>>>(A, link_off, link_vs, link_rel, link_roff, need); g_launches++;
+    if ((rc = LAUNCH(batch_links_kernel, static_cast<unsigned>((nf + 1 + 255) / 256), 256, 0, st, A, link_off, link_vs, link_rel, link_roff, need))) return rc;
     if ((rc = select_flagged(g->p_scan_tmp, need, ulist, nu, static_cast<int>(n), st))) return rc;
     CUDA_TRY(cudaMemsetAsync(t_cnt, 0, static_cast<size_t>(nu_max + 2) * 8, st));
-    if (nu_max) { batch_template_counts_kernel<<<static_cast<unsigned>((nu_max + 255) / 256), 256, 0, st>>>(A, ulist, nu, t_cnt); g_launches++; }
+    if (nu_max) if ((rc = LAUNCH(batch_template_counts_kernel, static_cast<unsigned>((nu_max + 255) / 256), 256, 0, st, A, ulist, nu, t_cnt))) return rc;
     if ((rc = scan_i64(g->p_scan_tmp, t_cnt, t_off, nu_max + 1, st))) return rc;
     int64_t TR = 0;
     CUDA_TRY(cudaMemcpyAsync(&TR, t_off + nu_max, 8, cudaMemcpyDeviceToHost, st));
@@ -1694,9 +1696,10 @@ static int paths_run(abb_graph *g, const int32_t *h_findings, const int32_t *d_f
     ENS(pt_row, (TR + 2) * 16); ENS(pt_rel, (TR + 2) * 2);
     if (rc) return rc;
     int64_t *t_off_node = g->pt_off_node.as<int64_t>();
-    if (nu_max) { batch_templates_kernel<<<warp_grid(g, nu_max), 256, 0, st>>>(A, ulist, nu, t_off, t_off_node, g->pt_row.as<int4>(), g->pt_rel.as<int8_t>()); g_launches++; }
-    if (NL) { batch_link_toff_kernel<<<static_cast<unsigned>((NL + 255) / 256), 256, 0, st>>>(NL, link_vs, t_off_node, link_toff); g_launches++; }
-    CUDA_TRY(cudaGetLastError());
+    if (nu_max)
+        if ((rc = LAUNCH(batch_templates_kernel, warp_grid(g, nu_max), 256, 0, st, A, ulist, nu, t_off, t_off_node, g->pt_row.as<int4>(), g->pt_rel.as<int8_t>())))
+            return rc;
+    if (NL) if ((rc = LAUNCH(batch_link_toff_kernel, static_cast<unsigned>((NL + 255) / 256), 256, 0, st, NL, link_vs, t_off_node, link_toff))) return rc;
     CUDA_TRY(cudaEventRecord(g->ev[3], st));
     g->paths_timed = true;
     const size_t n1 = static_cast<size_t>(nf) + 1;
@@ -1784,7 +1787,7 @@ static int paths_rank(abb_graph *g, const int32_t *findings, int64_t n_findings,
     PathsArgs A = g->paths_args;
     RankArgs RA{d_base.as<int32_t>(), d_tab.as<uint32_t>(), d_ncu.as<int32_t>(), d_ntu.as<int32_t>(), k1.as<unsigned long long>(), v1.as<uint32_t>(),
                 d_focus.as<uint8_t>(), need};
-    rank_keys_kernel<<<row_grid(g, rank_keys_kernel, g->rank_keys_grid), ROW_THREADS, 0, st>>>(A, RA); g_launches++;
+    if ((rc = LAUNCH(rank_keys_kernel, row_grid(g, rank_keys_kernel, g->rank_keys_grid), ROW_THREADS, 0, st, A, RA))) return rc;
     // sort input: every row (k1, v1), or the matched rows compacted into (k2, v2); the sorted pairs land in the other pair
     unsigned long long *key_in = k1.as<unsigned long long>(), *key_out = k2.as<unsigned long long>();
     uint32_t *row_in = v1.as<uint32_t>(), *row_out = v2.as<uint32_t>();
@@ -1798,8 +1801,9 @@ static int paths_rank(abb_graph *g, const int32_t *findings, int64_t n_findings,
         CUDA_TRY(cudaStreamSynchronize(st));
         r->matched = M;
         if (M == 0 || std::min(limit, M - std::min(offset, M)) == 0) { *out = r.release(); return ABB_OK; }
-        gather_keys_kernel<<<static_cast<unsigned>((M + 255) / 256), 256, 0, st>>>(k1.as<unsigned long long>(), v2.as<uint32_t>(), M, k2.as<unsigned long long>());
-        g_launches++;
+        if ((rc = LAUNCH(gather_keys_kernel, static_cast<unsigned>((M + 255) / 256), 256, 0, st, k1.as<unsigned long long>(), v2.as<uint32_t>(), M,
+                         k2.as<unsigned long long>())))
+            return rc;
         std::swap(key_in, key_out); std::swap(row_in, row_out);
     }
     const int64_t M = r->matched;
@@ -1816,8 +1820,9 @@ static int paths_rank(abb_graph *g, const int32_t *findings, int64_t n_findings,
     if (!rc) rc = o_row.alloc(static_cast<size_t>(count) * 8);
     if (rc) return rc;
     A.io.hops = o_hops.as<int32_t>(); A.io.rels = o_rels.as<int8_t>(); A.io.ncred = o_nc.as<int32_t>(); A.io.ntool = o_nt.as<int32_t>(); A.io.row_cap = count;
-    rank_gather_kernel<<<static_cast<unsigned>((count + 255) / 256), 256, 0, st>>>(A, RA, row_out, first, count, o_rank.as<uint32_t>(), o_row.as<int64_t>());
-    g_launches++;
+    if ((rc = LAUNCH(rank_gather_kernel, static_cast<unsigned>((count + 255) / 256), 256, 0, st, A, RA, row_out, first, count, o_rank.as<uint32_t>(),
+                     o_row.as<int64_t>())))
+        return rc;
     r->hops.resize(static_cast<size_t>(count) * 4); r->rels.resize(static_cast<size_t>(count) * 4); r->ncred.resize(count); r->ntool.resize(count);
     r->risk_rank.resize(count); r->row.resize(count);
     cudaError_t ce = cudaGetLastError();
@@ -1947,7 +1952,7 @@ extern "C" int abb_finding_context_host(abb_graph *g, int32_t max_depth, const i
     const unsigned grid = warp_grid(g, (nq + 31) / 32);
     CUDA_TRY(cudaEventRecord(g->cx_ev[0], cs));
     CUDA_TRY(cudaMemsetAsync(A.cnt, 0, q1 * 8, cs));
-    if (nq) { context_kernel<false><<<grid, 256, 0, cs>>>(A); g_launches++; }
+    if (nq) if ((rc = LAUNCH(context_kernel<false>, grid, 256, 0, cs, A))) { drain(); return rc; }
     if ((rc = scan_i64(g->p_scan_tmp, A.cnt, g->cx_start.as<int64_t>(), nq + 1, cs))) { drain(); return rc; }
     CUDA_TRY(cudaEventRecord(g->cx_ev[1], cs));
     // the impact walk, unchanged, into the device arena
@@ -1967,7 +1972,7 @@ extern "C" int abb_finding_context_host(abb_graph *g, int32_t max_depth, const i
     // fill pass and its copies on paths_stream, the walk's per-finding arrays on the main stream
     A.src = g->cx_src.as<int32_t>();
     CUDA_TRY(cudaEventRecord(g->cx_ev[2], cs));
-    if (nq) { context_kernel<true><<<grid, 256, 0, cs>>>(A); g_launches++; }
+    if (nq) if ((rc = LAUNCH(context_kernel<true>, grid, 256, 0, cs, A))) { drain(); return rc; }
     CUDA_TRY(cudaEventRecord(g->cx_ev[3], cs));
     Readback d2h{cs, &r->d2h, cudaGetLastError()};
     d2h(r->start, g->cx_start.p, q * 8); d2h(r->bcnt, g->cx_bcnt.p, q * CTX_BUCKETS * 4); d2h(r->src, g->cx_src.p, static_cast<size_t>(total) * 4);
