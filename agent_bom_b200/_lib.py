@@ -226,6 +226,8 @@ EXPORTS = {
     "abb_delta_build_host": (C.c_int, [vp, vp, vp, vp, vp, vp]),
     "abb_delta_result_free": (None, [vp]),
     "abb_delta_fetch_host": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "abb_delta_shared_host": (C.c_int, [vp, vp]),
+    "abb_delta_shared_fetch_host": (C.c_int, [vp, vp, vp]),
     "abb_lookup_table_host": (C.c_int, [vp, i32, vp, i64, vp, vp, vp, vp]),
     "abb_lookup_table_bytes": (i64, [vp]),
     "abb_lookup_edges_host": (C.c_int, [vp, i64, vp, vp, vp]),
@@ -241,6 +243,10 @@ EXPORTS = {
     "abb_compliance_table_host": (C.c_int, [vp, i32, vp, vp, vp, i32, vp, vp, i32, vp, i32, i32, i32, vp]),
     "abb_compliance_table_bytes": (i64, [vp]),
     "abb_compliance_fetch_host": (C.c_int, [vp, vp, vp, vp, vp, vp]),
+    "abb_lifecycle_build_host": (C.c_int, [C.c_int, i64, vp, vp, vp, vp, vp, vp, i64, i64, i64, C.POINTER(vp), vp]),
+    "abb_lifecycle_active_host": (C.c_int, [vp, i32, vp, vp, vp]),
+    "abb_lifecycle_bytes": (i64, [vp]),
+    "abb_lifecycle_free": (None, [vp]),
 }
 
 _lock = threading.Lock()

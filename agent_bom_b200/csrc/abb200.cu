@@ -37,6 +37,7 @@
 #include "lookup.cuh"
 #include "search.cuh"
 #include "compliance.cuh"
+#include "lifecycle.cuh"
 
 using namespace abb;
 
@@ -2000,3 +2001,4 @@ extern "C" int abb_finding_context_host(abb_graph *g, int32_t max_depth, const i
 #include "lookup_host.inl"
 #include "search_host.inl"
 #include "compliance_host.inl"
+#include "lifecycle_host.inl"

@@ -10,7 +10,8 @@
 //   - edge keys: one 64-bit key per original edge (forward entry, reversed bit clear), urank(src) << 33 | urank(tgt) << 6 |
 //     relrank, radix-sorted per graph.  Ascending keys are sorted() over (source, target, relationship) string tuples;
 //   - edge set difference: every sorted key binary-searches the other graph's sorted keys.  A shared key compares the
-//     bidirectional and traversable flags and, when both graphs carry a weight column, the weight (f64 ==).
+//     bidirectional and traversable flags and, when both graphs carry a weight column, the weight (f64 ==);
+//   - shared edges (on request): the sorted keys of the new graph that have a partner, as (new edge, old edge) pairs in key order.
 #pragma once
 #include <cstdint>
 
@@ -131,6 +132,12 @@ __global__ void delta_edge_diff_kernel(int64_t na, const unsigned long long *__r
             partner[k] = pe;
         }
     }
+}
+
+// flag[k] = 1 when sorted key k of the new graph has a partner in the old graph (a shared key).
+__global__ void delta_shared_flag_kernel(int64_t n, const int32_t *__restrict__ partner, uint8_t *__restrict__ flag) {
+    for (int64_t k = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; k < n; k += static_cast<int64_t>(gridDim.x) * blockDim.x)
+        flag[k] = partner[k] >= 0;
 }
 
 // out[j] = a[pos[j]], or b[a[pos[j]]] when b is given; flag_out[j] = flag[pos[j]] when both are given.

@@ -599,11 +599,12 @@ class DeviceGraph:
         with self._use() as h:
             return int(_lib.load().abb_delta_table_bytes(h))
 
-    def diff(self, old: "DeviceGraph", relmap_old, relmap_new) -> dict[str, np.ndarray]:
+    def diff(self, old: "DeviceGraph", relmap_old, relmap_new, shared: bool = False) -> dict[str, np.ndarray]:
         """Diff ``old`` -> this graph on the device (``abb_delta_build_host`` + ``abb_delta_fetch_host``); both need delta tables.
         Returns ``nodes_added`` (this graph's indices) / ``nodes_removed`` (old's) in id order, ``changed_new`` / ``changed_old`` /
         ``changed_flag`` node pairs in id order, ``edges_added`` / ``edges_removed`` edge indices and ``echanged_new`` /
-        ``echanged_old`` edge pairs in (source, target, relationship) order."""
+        ``echanged_old`` edge pairs in (source, target, relationship) order.  ``shared`` adds ``shared_new`` / ``shared_old``, the
+        edge pairs whose key both graphs hold, in key order (``abb_delta_shared_host``)."""
         rm_old = np.zeros(64, np.uint8)
         rm_new = np.zeros(64, np.uint8)
         rm_old[: len(relmap_old)] = relmap_old
@@ -620,6 +621,11 @@ class DeviceGraph:
                    "edges_removed": np.empty(er, np.int32), "echanged_new": np.empty(ec, np.int32), "echanged_old": np.empty(ec, np.int32)}
             _lib.check(lib.abb_delta_fetch_host(res, *(out[k].ctypes.data for k in ("nodes_added", "nodes_removed", "changed_new", "changed_old", "changed_flag",
                                                                                      "edges_added", "edges_removed", "echanged_new", "echanged_old"))))
+            if shared:
+                n = C.c_int64()
+                _lib.check(lib.abb_delta_shared_host(res, C.byref(n)))
+                out["shared_new"], out["shared_old"] = np.empty(n.value, np.int32), np.empty(n.value, np.int32)
+                _lib.check(lib.abb_delta_shared_fetch_host(res, out["shared_new"].ctypes.data, out["shared_old"].ctypes.data))
         finally:
             lib.abb_delta_result_free(res)
         return out
@@ -822,3 +828,77 @@ def group_union(member_off, members, item_off, items, w0=None, w1=None, *, devic
         return off, out, g0, g1, float(lib.abb_union_result_ms(res))
     finally:
         lib.abb_union_result_free(res)
+
+
+class EdgeHistory:
+    """One tenant's edge history on one device (``abb_lifecycle_build_host``), freed by ``close()`` or the destructor.  Calls are
+    thread-safe: the library serialises calls on one history, and ``close()`` waits for calls in flight."""
+
+    ID_LIMIT = 1 << 27
+
+    def __init__(self, src, tgt, rel, created, valid_from, valid_to, n_ids: int, n_rels: int, *, device: int = 0, id_limit: int | None = None):
+        cols = [_i32(a) for a in (src, tgt, rel, created, valid_from, valid_to)]
+        n = cols[0].shape[0]
+        if any(c.shape != (n,) for c in cols):
+            raise ValueError("edge history columns have different lengths")
+        lib = _lib.load()
+        _lib.require_device()
+        h, n_seg = _vp(), C.c_int64()
+        _lib.check(lib.abb_lifecycle_build_host(device, n, *(c.ctypes.data for c in cols), int(n_ids), int(n_rels),
+                                                self.ID_LIMIT if id_limit is None else int(id_limit), C.byref(h), C.byref(n_seg)))
+        self._h = h
+        self.device = device
+        self.n_rows = n
+        self.n_keys = int(n_seg.value)
+        self._lock = threading.Condition()
+        self._users = 0
+
+    def close(self) -> None:
+        with self._lock:
+            if not self._h:
+                return
+            while self._users:
+                self._lock.wait()
+            h, self._h = self._h, None
+        _lib.load().abb_lifecycle_free(h)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _enter(self):
+        with self._lock:
+            if not self._h:
+                raise RuntimeError("EdgeHistory is closed")
+            self._users += 1
+            return self._h
+
+    def _exit(self) -> None:
+        with self._lock:
+            self._users -= 1
+            if not self._users:
+                self._lock.notify_all()
+
+    def active(self, r: int, timing: dict | None = None) -> np.ndarray:
+        """Row indices of the last version of each key active at rank ``r`` (``abb_lifecycle_active_host``), in key order.
+        ``timing`` (optional) receives the device milliseconds as ``device_ms``."""
+        out = np.empty(max(self.n_keys, 1), np.int32)
+        count, ms = C.c_int64(), C.c_float()
+        h = self._enter()
+        try:
+            _lib.check(_lib.load().abb_lifecycle_active_host(h, int(r), out.ctypes.data, C.byref(count), C.byref(ms)))
+        finally:
+            self._exit()
+        if timing is not None:
+            timing["device_ms"] = float(ms.value)
+        return out[: count.value]
+
+    @property
+    def nbytes(self) -> int:
+        h = self._enter()
+        try:
+            return int(_lib.load().abb_lifecycle_bytes(h))
+        finally:
+            self._exit()

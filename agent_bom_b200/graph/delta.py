@@ -15,6 +15,9 @@ node row and a ``(source, target, relationship)`` tuple for every edge row of bo
 - edge rows whose endpoints are not both nodes of their scan are stored but not loaded as graph edges; one SQL query per scan
   finds them and they are merged into the answer on the host;
 - dicts are built only for the rows returned.
+
+``changed_edges_between_scans`` reuses the same device diff and edge correction, plus the shared edge pairs the device already
+matched (``abb_delta_shared_host``), and returns full rows for the added, removed and unchanged keys.
 """
 
 from __future__ import annotations
@@ -118,8 +121,9 @@ def delta_table(graph) -> DeltaTable:
     return t
 
 
-def device_diff(old, new) -> dict[str, np.ndarray]:
-    """The device's answer for ``old`` -> ``new`` (``DeviceGraph.diff``), with the relationship slots of both graphs ranked together."""
+def device_diff(old, new, shared: bool = False) -> dict[str, np.ndarray]:
+    """The device's answer for ``old`` -> ``new`` (``DeviceGraph.diff``), with the relationship slots of both graphs ranked together;
+    ``shared`` adds the edge pairs whose key both graphs hold."""
     to, tn = delta_table(old), delta_table(new)
     union = sorted(set(to.rel_names) | set(tn.rel_names))
     if len(union) > REL_SLOTS:
@@ -128,7 +132,10 @@ def device_diff(old, new) -> dict[str, np.ndarray]:
     with _lock:
         to.ensure_device(old)
         tn.ensure_device(new)
-    return new.device_graph.diff(old.device_graph, [rank[s] for s in to.rel_names], [rank[s] for s in tn.rel_names])
+    relmaps = [rank[s] for s in to.rel_names], [rank[s] for s in tn.rel_names]
+    if shared:
+        return new.device_graph.diff(old.device_graph, *relmaps, shared=True)
+    return new.device_graph.diff(old.device_graph, *relmaps)
 
 
 # ── reference row rules (db/graph_store.py:680-689, 741-773), restated ──
@@ -218,6 +225,44 @@ def _holds_unloaded_edges(graph) -> bool:
     return isinstance(graph, SnapshotGraph)
 
 
+def _edge_sql(conn, tenant: str, old, new, old_scan: str, new_scan: str, nodeless: bool = False):
+    """The SQL half of the edge comparison: shared keys with a differing stored column, and each scan's rows the loader dropped.
+    ``nodeless``: a graph without nodes stands for a named scan whose stored edge rows (if any) all lack their endpoints."""
+    def unloaded(g, scan):
+        if _holds_unloaded_edges(g) or (nodeless and scan and not g.nodes):
+            return unloaded_edge_keys(conn, tenant, scan)
+        return set()
+
+    return rich_edge_candidates(conn, tenant, old_scan, new_scan), unloaded(old, old_scan), unloaded(new, new_scan)
+
+
+def _edge_changes(conn, tenant: str, old, new, old_scan: str, new_scan: str, d: dict[str, np.ndarray], sql) -> dict[str, Any]:
+    """The edge half of a diff: ``added`` / ``removed`` keys and ``changed`` {before, after} rows in key order, from the device's
+    lists corrected by the stored rows the loaded graphs do not hold; with ``d["shared_new"]`` also the ``unchanged`` keys (every key
+    both scans store, minus the changed ones)."""
+    rich_edges, go, gn = sql
+    e_add = [_edge_key(new, e) for e in d["edges_added"].tolist()]
+    e_rem = [_edge_key(old, e) for e in d["edges_removed"].tolist()]
+    e_chg = {_edge_key(new, e) for e in d["echanged_new"].tolist()}
+    shared_unloaded: list[tuple[str, str, str]] = []
+    if go or gn:
+        in_old = set(_edge_rows(conn, tenant, old_scan, sorted(gn)))
+        in_new = set(_edge_rows(conn, tenant, new_scan, sorted(go)))
+        shared_unloaded = sorted((gn & in_old) | (go & in_new))
+        e_add = sorted([k for k in e_add if k not in go] + [k for k in gn if k not in in_old])
+        e_rem = sorted([k for k in e_rem if k not in gn] + [k for k in go if k not in in_new])
+    check_e = sorted((set(rich_edges) | set(shared_unloaded) | e_chg))
+    before = _edge_rows(conn, tenant, old_scan, check_e)
+    after = _edge_rows(conn, tenant, new_scan, check_e)
+    changed_keys = [k for k in check_e if k in before and k in after and (k in e_chg or edge_fingerprint(before[k]) != edge_fingerprint(after[k]))]
+    out = {"added": e_add, "removed": e_rem, "changed": [{"before": before[k], "after": after[k]} for k in changed_keys]}
+    if "shared_new" in d:
+        gone = set(changed_keys)
+        shared = {_edge_key(new, e) for e in d["shared_new"].tolist()} | set(shared_unloaded)
+        out["unchanged"] = sorted(k for k in shared if k not in gone)
+    return out
+
+
 def snapshot_diff(old, new, *, db_path=None, tenant_id: str | None = None, timings: dict | None = None) -> dict[str, Any]:
     """The body of the reference ``diff_snapshots(old.scan_id, new.scan_id)`` for two snapshots persisted in ``db_path`` (default: the
     graphs' own database), with ``old`` and ``new`` as their device graphs.  ``timings`` (optional) receives the seconds of each stage."""
@@ -239,9 +284,7 @@ def snapshot_diff(old, new, *, db_path=None, tenant_id: str | None = None, timin
     conn.row_factory = sqlite3.Row
     try:
         rich_nodes = rich_node_candidates(conn, tenant, old_scan, new_scan)
-        rich_edges = rich_edge_candidates(conn, tenant, old_scan, new_scan)
-        go = unloaded_edge_keys(conn, tenant, old_scan) if _holds_unloaded_edges(old) else set()
-        gn = unloaded_edge_keys(conn, tenant, new_scan) if _holds_unloaded_edges(new) else set()
+        sql = _edge_sql(conn, tenant, old, new, old_scan, new_scan)
         t["sql_s"] = time.perf_counter() - t0
         t0 = time.perf_counter()
         oids, nids = old.csr.node_ids, new.csr.node_ids
@@ -257,28 +300,78 @@ def snapshot_diff(old, new, *, db_path=None, tenant_id: str | None = None, timin
             a, b = _node_rows(conn, tenant, old_scan, check), _node_rows(conn, tenant, new_scan, check)
             changed.update(nid for nid in check if nid in a and nid in b and a[nid] != b[nid])
         # edges: device lists in key order, corrected by the stored rows the loaded graphs do not hold
-        e_add = [_edge_key(new, e) for e in d["edges_added"].tolist()]
-        e_rem = [_edge_key(old, e) for e in d["edges_removed"].tolist()]
-        e_chg = {_edge_key(new, e) for e in d["echanged_new"].tolist()}
-        shared_unloaded: list[tuple[str, str, str]] = []
-        if go or gn:
-            in_old = set(_edge_rows(conn, tenant, old_scan, sorted(gn)))
-            in_new = set(_edge_rows(conn, tenant, new_scan, sorted(go)))
-            shared_unloaded = sorted((gn & in_old) | (go & in_new))
-            e_add = sorted([k for k in e_add if k not in go] + [k for k in gn if k not in in_old])
-            e_rem = sorted([k for k in e_rem if k not in gn] + [k for k in go if k not in in_new])
-        check_e = sorted((set(rich_edges) | set(shared_unloaded) | e_chg))
-        before = _edge_rows(conn, tenant, old_scan, check_e)
-        after = _edge_rows(conn, tenant, new_scan, check_e)
-        edges_changed = [{"before": before[k], "after": after[k]} for k in check_e
-                         if k in before and k in after and (k in e_chg or edge_fingerprint(before[k]) != edge_fingerprint(after[k]))]
+        edges = _edge_changes(conn, tenant, old, new, old_scan, new_scan, d, sql)
         body = {
             "nodes_added": [new_rows[nid] for nid in added_ids],
             "nodes_removed": [old_rows[nid] for nid in removed_ids],
             "nodes_changed": sorted(changed),
-            "edges_added": e_add,
-            "edges_removed": e_rem,
-            "edges_changed": edges_changed,
+            "edges_added": edges["added"],
+            "edges_removed": edges["removed"],
+            "edges_changed": edges["changed"],
+        }
+        t["response_s"] = time.perf_counter() - t0
+    finally:
+        conn.close()
+    if timings is not None:
+        timings.update(t)
+    return body
+
+
+_FULL_SCAN = 2000      # above this many keys one pass over the scan's rows beats keyed lookups
+
+
+def _rows_of(conn, tenant: str, scan: str, keys: list[tuple[str, str, str]]) -> dict[tuple[str, str, str], dict[str, Any]]:
+    """Full history rows of ``keys`` in one scan: keyed lookups for a few, one pass over the scan's rows for many."""
+    if len(keys) <= _FULL_SCAN:
+        return _edge_rows(conn, tenant, scan, keys)
+    want = set(keys)
+    out: dict[tuple[str, str, str], dict[str, Any]] = {}
+    for row in conn.execute("SELECT * FROM graph_edges WHERE scan_id = ? AND tenant_id = ?", (scan, tenant)):
+        k = (row["source_id"], row["target_id"], row["relationship"])
+        if k in want:
+            out[k] = edge_history_row(row)
+    return out
+
+
+def changed_edges_between_scans(old, new, *, db_path=None, tenant_id: str | None = None, timings: dict | None = None) -> dict[str, Any]:
+    """The body of the reference ``changed_edges_between_scans(old.scan_id, new.scan_id)`` (db/graph_store.py:799-841) for two
+    snapshots persisted in ``db_path``, with ``old`` and ``new`` as their device graphs.  The key sets come from the device diff (its
+    shared pairs give the unchanged edges) corrected as ``snapshot_diff`` corrects them; ``edges_changed`` is exactly the diff's.
+    Rows are built only for the keys returned.  ``timings`` (optional) receives the seconds of each stage."""
+    import time
+
+    from .snapshot import normalize_graph_tenant_id
+
+    db_path = db_path or getattr(new, "db_path", None) or getattr(old, "db_path", None)
+    if not db_path:
+        raise ValueError("changed_edges_between_scans compares persisted snapshots: pass db_path")
+    tenant = normalize_graph_tenant_id(new.tenant_id if tenant_id is None else tenant_id)
+    old_scan, new_scan = old.scan_id or "", new.scan_id or ""
+    t = {}
+    t0 = time.perf_counter()
+    d = device_diff(old, new, shared=True)
+    t["device_s"] = time.perf_counter() - t0
+    t0 = time.perf_counter()
+    conn = sqlite3.connect(f"file:{db_path}?mode=ro", uri=True, timeout=10)
+    conn.row_factory = sqlite3.Row
+    try:
+        conn.execute("BEGIN")          # one read transaction: every row below comes from one state of the database
+        sql = _edge_sql(conn, tenant, old, new, old_scan, new_scan, nodeless=True)
+        t["sql_s"] = time.perf_counter() - t0
+        t0 = time.perf_counter()
+        edges = _edge_changes(conn, tenant, old, new, old_scan, new_scan, d, sql)
+        new_rows = _rows_of(conn, tenant, new_scan, sorted(set(edges["added"]) | set(edges["unchanged"])))
+        old_rows = _rows_of(conn, tenant, old_scan, edges["removed"])
+        conn.rollback()
+        body = {
+            "scan_id_old": old_scan,
+            "scan_id_new": new_scan,
+            "edges_added": [new_rows[k] for k in edges["added"]],
+            "edges_removed": [old_rows[k] for k in edges["removed"]],
+            "edges_changed": edges["changed"],
+            "edges_unchanged": [new_rows[k] for k in edges["unchanged"]],
+            "summary": {"added": len(edges["added"]), "removed": len(edges["removed"]), "changed": len(edges["changed"]),
+                        "unchanged": len(edges["unchanged"])},
         }
         t["response_s"] = time.perf_counter() - t0
     finally:

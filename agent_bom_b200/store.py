@@ -47,10 +47,13 @@ class B200GraphStore:
     """``max_graphs`` bounds the snapshot cache: every cached snapshot pins a device CSR plus its walk workspace in HBM, so the
     least recently used one is dropped (and freed once no caller is inside it) when a new snapshot would exceed the bound."""
 
-    def __init__(self, inner=None, *, device: int = 0, max_graphs: int = 4):
+    def __init__(self, inner=None, *, device: int = 0, max_graphs: int = 4, max_histories: int = 4):
+        from .graph.lifecycle import HistoryCache
+
         self._inner = inner
         self._device = device
         self._max_graphs = max(1, int(max_graphs))
+        self._histories = HistoryCache(max_histories, device=device)      # tenant edge histories of active_edges_at
         self._lock = threading.RLock()
         self._graphs: "dict[tuple[str, str], UnifiedGraph]" = {}     # insertion order = recency (re-inserted on use)
         self._latest: dict[str, str] = {}                             # only when there is no inner store to ask
@@ -235,6 +238,41 @@ class B200GraphStore:
             return g if g is not None else UnifiedGraph(scan_id=scan_id, tenant_id=tenant, device=self._device)
 
         return snapshot_diff(snapshot(scan_id_old), snapshot(scan_id_new), db_path=db_path, tenant_id=tenant)
+
+    def changed_edges_between_scans(self, scan_id_old: str, scan_id_new: str, *, tenant_id: str = "") -> dict[str, Any]:
+        """The body of ``GET /v1/graph/edges/changes`` (reference db/graph_store.py:799-841): full rows of the edges added, removed
+        and unchanged, the changed pairs and their counts, from the device diff of the two cached snapshots when the inner store is
+        SQLite-backed; otherwise the inner store's own method.  A blank or missing scan id is an empty snapshot, as for
+        ``diff_snapshots``."""
+        from .graph.delta import changed_edges_between_scans
+
+        db = self._sqlite_db()
+        if db is None:
+            inner = getattr(self._inner, "changed_edges_between_scans", None) if self._inner is not None else None
+            if inner is None:
+                raise B200UnsupportedOperationError("B200GraphStore has no inner store to serve changed_edges_between_scans()")
+            return inner(scan_id_old, scan_id_new, tenant_id=tenant_id)
+        tenant = normalize_tenant(tenant_id)
+
+        def snapshot(scan_id: str) -> UnifiedGraph:
+            g = self._graph(tenant, scan_id) if scan_id else None
+            return g if g is not None else UnifiedGraph(scan_id=scan_id, tenant_id=tenant, device=self._device)
+
+        return changed_edges_between_scans(snapshot(scan_id_old), snapshot(scan_id_new), db_path=db, tenant_id=tenant)
+
+    def active_edges_at(self, at: str, *, tenant_id: str = "") -> list[dict[str, Any]]:
+        """The body of ``GET /v1/graph/edges/active?at=`` (reference db/graph_store.py:775-796): the latest version of each edge key
+        active at ``at``, in key order, selected on the device from the tenant's cached edge history when the inner store is
+        SQLite-backed; otherwise the inner store's own method.  The history is rebuilt whenever the tenant's snapshots change."""
+        from .graph.lifecycle import active_edges_at
+
+        db = self._sqlite_db()
+        if db is None:
+            inner = getattr(self._inner, "active_edges_at", None) if self._inner is not None else None
+            if inner is None:
+                raise B200UnsupportedOperationError("B200GraphStore has no inner store to serve active_edges_at()")
+            return inner(at, tenant_id=tenant_id)
+        return active_edges_at(self._histories, db, at, tenant_id=tenant_id)
 
     # ── record lookups (GPU over the snapshot cache; SQLite only by key) ──
     def _sqlite_db(self) -> str | None:

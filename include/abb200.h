@@ -550,6 +550,12 @@ int abb_delta_build_host(abb_graph *old_g, abb_graph *new_g, const uint8_t *relm
 void abb_delta_result_free(abb_delta_result *r);
 int abb_delta_fetch_host(const abb_delta_result *r, int32_t *nodes_added, int32_t *nodes_removed, int32_t *changed_new, int32_t *changed_old,
                          uint8_t *changed_flag, int32_t *edges_added, int32_t *edges_removed, int32_t *echanged_new, int32_t *echanged_old);
+/* Shared edges of a diff (changed_edges_between_scans, :799-841, needs the unchanged ones too): abb_delta_shared_host finds, once per
+ * result, the new graph's edges whose (source, target, relationship) key the old graph also has and writes their number to
+ * *count_out; abb_delta_shared_fetch_host copies them as (new edge, old edge) index pairs in key order.  Neither changes what
+ * abb_delta_fetch_host returns. */
+int abb_delta_shared_host(abb_delta_result *r, int64_t *count_out);
+int abb_delta_shared_fetch_host(const abb_delta_result *r, int32_t *shared_new, int32_t *shared_old);
 
 /* ---- snapshot lookups -----------------------------------------------------------------------------------------
  * Replace the per-request edge-row scans of edges_for_node_ids, node_context and the unfiltered snapshot_stats
@@ -627,6 +633,25 @@ int abb_compliance_table_host(abb_graph *g, int32_t n, const int32_t *row_text, 
                               int32_t n_types, int64_t *sizes_out);
 int64_t abb_compliance_table_bytes(const abb_graph *g);          /* device bytes of the compliance table, 0 when none */
 int abb_compliance_fetch_host(abb_graph *g, int64_t *sev_runs, int64_t *type_runs, int64_t *tag_runs, int64_t *node_count, int32_t *node_rows);
+
+/* ---- edge lifecycle: versions active at a timestamp -------------------------------------------------------------
+ * Replaces the row-dict build and keyed selection of active_edges_at (agent_bom/db/graph_store.py:775-796).
+ * abb_lifecycle_build_host builds one tenant's edge history on `device`: per stored edge row, in (created_at, scan_id) order,
+ * the ranks of its source and target id (< n_ids) and relationship (< n_rels) in sorted dictionaries, and the ranks of its
+ * snapshot's created_at, its effective valid_from and its valid_to in one sorted dictionary of timestamp strings (0x7FFFFFFF:
+ * absent; an absent valid_from is never <= at, an absent valid_to is open).  It fails when n_ids exceeds id_limit (at most
+ * 2^27) or n_rels exceeds 2^10.  The history is owned by the caller (abb_lifecycle_free) and *n_seg_out receives its number of
+ * distinct keys.  abb_lifecycle_active_host takes r, the number of dictionary strings <= at, and writes to rows_out (room for
+ * n_seg entries) the row index of the last version of each key whose created_at and valid_from are <= at and whose valid_to is
+ * > at, in (source, target, relationship) order; *count_out receives their number and ms_out (optional) the device time.
+ * Calls on one history are serialised.  All pointers are host memory. */
+typedef struct abb_lifecycle_history abb_lifecycle_history;
+int abb_lifecycle_build_host(int device, int64_t n_rows, const int32_t *src, const int32_t *tgt, const int32_t *rel, const int32_t *created,
+                             const int32_t *valid_from, const int32_t *valid_to, int64_t n_ids, int64_t n_rels, int64_t id_limit,
+                             abb_lifecycle_history **out, int64_t *n_seg_out);
+int abb_lifecycle_active_host(abb_lifecycle_history *h, int32_t r, int32_t *rows_out, int64_t *count_out, float *ms_out);
+int64_t abb_lifecycle_bytes(const abb_lifecycle_history *h);      /* device bytes of the history and its workspace */
+void abb_lifecycle_free(abb_lifecycle_history *h);
 
 #ifdef __cplusplus
 }
