@@ -247,6 +247,17 @@ EXPORTS = {
     "abb_lifecycle_active_host": (C.c_int, [vp, i32, vp, vp, vp]),
     "abb_lifecycle_bytes": (i64, [vp]),
     "abb_lifecycle_free": (None, [vp]),
+    "abb_hops_host": (C.c_int, [C.c_int, i32, i32, vp, vp, i32, vp, vp, vp, i32, vp, vp, i64, vp, vp, vp, vp, vp, vp, i64, C.POINTER(vp)]),
+    "abb_hops_result_counts": (None, [vp, vp]),
+    "abb_hops_result_times": (None, [vp, vp]),
+    "abb_hops_result_disc_sig": (vp, [vp]),
+    "abb_hops_result_disc_occ": (vp, [vp]),
+    "abb_hops_result_disc_hop": (vp, [vp]),
+    "abb_hops_result_disc_parent": (vp, [vp]),
+    "abb_hops_result_entry_server": (vp, [vp]),
+    "abb_hops_result_entry_parent": (vp, [vp]),
+    "abb_hops_result_cred": (vp, [vp]),
+    "abb_hops_result_free": (None, [vp]),
 }
 
 _lock = threading.Lock()

@@ -38,6 +38,7 @@
 #include "search.cuh"
 #include "compliance.cuh"
 #include "lifecycle.cuh"
+#include "hops.cuh"
 
 using namespace abb;
 
@@ -2002,3 +2003,4 @@ extern "C" int abb_finding_context_host(abb_graph *g, int32_t max_depth, const i
 #include "search_host.inl"
 #include "compliance_host.inl"
 #include "lifecycle_host.inl"
+#include "hops_host.inl"

@@ -653,6 +653,33 @@ int abb_lifecycle_active_host(abb_lifecycle_history *h, int32_t r, int32_t *rows
 int64_t abb_lifecycle_bytes(const abb_lifecycle_history *h);      /* device bytes of the history and its workspace */
 void abb_lifecycle_free(abb_lifecycle_history *h);
 
+/* ---- multi-hop blast-radius expansion --------------------------------------------------------------------------
+ * Replaces the per-blast-radius BFS of expand_blast_radius_hops (agent_bom/scanners/blast_radius.py:16-97).  Inputs, all host
+ * memory with int64 offsets: name -> servers (name_srv_off[n_names + 1], name_srv; the last agent object of a name), server ->
+ * agent occurrences (srv_occ_off[n_servers + 1]; per occurrence its name and credential set), credential sets (cset_off,
+ * cset_cred), and per signature the agent names and servers to mark visited and the first-level queue's servers (first_off,
+ * first_srv; global entry id = list position).  max_depth is the clamped depth, 2..5.  `batch` > 0 caps how many signatures
+ * are searched at once (0: as many as a quarter of free device memory allows).  The result (abb_hops_result_free) holds:
+ *   counts: {discoveries, entries of levels >= 2, credential keys, batches, batch size}; times: {upload, search, readback} ms;
+ *   per discovery, in (batch, level, signature, queue) order: signature, occurrence, hop and parent entry id;
+ *   per later entry, in the same order (global ids n_first, n_first + 1, ...): server and parent discovery id;
+ *   the sorted unique (signature << 32 | credential id) keys. */
+typedef struct abb_hops_result abb_hops_result;
+int abb_hops_host(int device, int32_t max_depth, int32_t n_names, const int64_t *name_srv_off, const int32_t *name_srv, int32_t n_servers,
+                  const int64_t *srv_occ_off, const int32_t *occ_name, const int32_t *occ_cset, int32_t n_csets, const int64_t *cset_off,
+                  const int32_t *cset_cred, int64_t n_sigs, const int64_t *mark_agent_off, const int32_t *mark_agent, const int64_t *mark_srv_off,
+                  const int32_t *mark_srv, const int64_t *first_off, const int32_t *first_srv, int64_t batch, abb_hops_result **out);
+void abb_hops_result_counts(const abb_hops_result *r, int64_t *out);
+void abb_hops_result_times(const abb_hops_result *r, double *out);
+const int32_t *abb_hops_result_disc_sig(const abb_hops_result *r);
+const int32_t *abb_hops_result_disc_occ(const abb_hops_result *r);
+const int32_t *abb_hops_result_disc_hop(const abb_hops_result *r);
+const int64_t *abb_hops_result_disc_parent(const abb_hops_result *r);
+const int32_t *abb_hops_result_entry_server(const abb_hops_result *r);
+const int64_t *abb_hops_result_entry_parent(const abb_hops_result *r);
+const unsigned long long *abb_hops_result_cred(const abb_hops_result *r);
+void abb_hops_result_free(abb_hops_result *r);
+
 #ifdef __cplusplus
 }
 #endif
