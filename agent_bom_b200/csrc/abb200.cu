@@ -280,12 +280,18 @@ struct Readback {
 };
 
 // ------------------------------------------------------------------ graph handle
+struct ClusterTable;      // clusters_host.inl
+struct DeltaTable;        // delta_host.inl
+struct LookupState;       // lookup_host.inl
+struct SearchState;       // search_host.inl
+struct ComplianceTable;   // compliance_host.inl
+
 struct abb_graph {
     int device = 0;
     GraphView v{};
     int64_t bytes = 0;
     int sm_count = 132;               // H100 SXM; set from the device in graph_finish_init
-    std::mutex mu;                    // serialises use of the shared workspace
+    mutable std::mutex mu;            // serialises use of the shared workspace and of the snapshot tables
     cudaStream_t stream = nullptr;    // host-API stream
     cudaStream_t copy_stream = nullptr;   // result copies that may overlap later kernels of the same call
     cudaStream_t paths_stream = nullptr;  // exposure-path pipeline of abb_exposure_host, run next to the walk
@@ -359,49 +365,18 @@ struct abb_graph {
     DevBuf cx_bcnt, cx_cnt, cx_start, cx_src;
     cudaEvent_t cx_staged = nullptr;
     cudaEvent_t cx_ev[4] = {nullptr, nullptr, nullptr, nullptr};
-    // graph-constant semantic-cluster tables (clusters_host.inl): each cluster's members in id order, its (cluster << 5 | rel) pairs and
-    // their counts; host copies of both segment offsets [K+1].  cl_k = -1 until built.
-    DevBuf cl_members, cl_rel_key, cl_rel_cnt;
-    std::vector<int64_t> cl_mem_off, cl_rel_off;
-    int64_t cl_k = -1;
-    // snapshot-diff tables (delta_host.inl): id bytes + offsets of every node, sorted-order permutation; per real node the label
-    // bytes + offsets, status / severity codes and risk; per original edge a relationship slot, flags and (optionally) weight.
-    // dl_real = -1 until built.
-    DevBuf dl_ids, dl_ioff, dl_perm, dl_lbl, dl_loff, dl_stat, dl_sev, dl_risk, dl_erel, dl_eflag, dl_w;
-    int32_t dl_real = -1;
-    int64_t dl_ne = 0;
-    bool dl_has_w = false;
+    // snapshot tables, one owner per feature, each type declared in its *_host.inl.  A null table is not built; a rebuild drops the old
+    // table, builds a new one aside and installs it only once every step has succeeded.  Read and replaced under mu.
+    std::unique_ptr<ClusterTable> clusters;
+    std::unique_ptr<DeltaTable> delta;
     int64_t dl_union_limit = DL_UNION_LIMIT;
-    // lookup table (lookup_host.inl): per original edge the rank of its relationship string among the graph's.  lk_ready = false until built.
-    // The lookup workspace (node list, entry offsets, edge bitmap and its scan, context keys, counter, cub temp) is reused under mu.
-    DevBuf lk_erel;
-    bool lk_ready = false;
-    DevBuf lk_nodes, lk_start, lk_bits, lk_cnt, lk_off, lk_keys, lk_keys2, lk_vals, lk_ctr, lk_tmp;
-    // search table (search_host.inl): per node the raw and token text with offsets, the rows a warp does not scan, severity, risk,
-    // label rank, entity-type / compliance / data-source codes, and the page order with its inverse.  sr_ready = false until built;
-    // sr_n = -1 until the text is stored.  The search workspace (flags, selection, counters, patterns and tables, cub temp) is
-    // reused under mu.
-    DevBuf sr_raw, sr_roff, sr_tok, sr_toff, sr_long, sr_sev, sr_risk, sr_label, sr_type, sr_cmp, sr_src, sr_order, sr_pos;
-    int32_t sr_n = -1, sr_types = 0, sr_ncmp = 0, sr_nsrc = 0;
-    int64_t sr_n_long = 0;
-    bool sr_ready = false;
-    DevBuf sr_flags, sr_sel, sr_ctr, sr_pat, sr_tmp;
-    // compliance table (compliance_host.inl): (framework, severity), (framework, type) and (framework, tag) runs as [4][u] int64
-    // (framework, code, count, first row), node_count per framework and the first node ids per framework.  cm_sizes: the three run
-    // counts and the node-id count.  cm_ready = false until built.
-    DevBuf cm_sev, cm_type, cm_tag, cm_count, cm_rows;
-    int64_t cm_sizes[4] = {0, 0, 0, 0};
-    int32_t cm_nfw = 0;
-    bool cm_ready = false;
+    std::unique_ptr<LookupState> lookup;
+    std::unique_ptr<SearchState> search;
+    std::unique_ptr<ComplianceTable> compliance;
     // graph arrays of an uploaded graph (an adopted graph's belong to the caller)
     std::vector<DevBuf> owned_arrays;
 
-    // Runs with the graph's device current (abb_graph_free); the DevBuf members free themselves after it.
-    ~abb_graph() {
-        for (cudaStream_t s : {stream, copy_stream, paths_stream}) if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); }
-        for (cudaEvent_t e : {ev_copy, ev_chunk_walked, ev_chunk_copied[0], ev_chunk_copied[1], ev[0], ev[1], ev[2], ev[3], cx_staged, cx_ev[0], cx_ev[1], cx_ev[2], cx_ev[3]})
-            if (e) cudaEventDestroy(e);
-    }
+    ~abb_graph();   // defined after the *_host.inl files, where the snapshot-table types are complete
 };
 
 struct DeviceGuard {
@@ -2004,3 +1979,10 @@ extern "C" int abb_finding_context_host(abb_graph *g, int32_t max_depth, const i
 #include "compliance_host.inl"
 #include "lifecycle_host.inl"
 #include "hops_host.inl"
+
+// Runs with the graph's device current (abb_graph_free); the DevBuf members and the snapshot tables free themselves after it.
+abb_graph::~abb_graph() {
+    for (cudaStream_t s : {stream, copy_stream, paths_stream}) if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); }
+    for (cudaEvent_t e : {ev_copy, ev_chunk_walked, ev_chunk_copied[0], ev_chunk_copied[1], ev[0], ev[1], ev[2], ev[3], cx_staged, cx_ev[0], cx_ev[1], cx_ev[2], cx_ev[3]})
+        if (e) cudaEventDestroy(e);
+}
