@@ -171,8 +171,8 @@ struct DevBuf {
     template <class T> T *as() const { return static_cast<T *>(p); }
 };
 
-// grows workspace buffer g->buf; needs `g` and `int rc` in scope and keeps the first error in rc
-#define ENS(buf, bytes) if (!rc) rc = g->buf.ensure(static_cast<size_t>(bytes))
+// grows workspace buffer `buf`; needs `int rc` in scope and keeps the first error in rc
+#define ENS(buf, bytes) if (!rc) rc = (buf).ensure(static_cast<size_t>(bytes))
 
 // One cub algorithm: `call(temp, bytes)` makes the cub call, once to size it and once to run it, so both share one argument list.
 // `tmp` grows to exactly what cub asks for; each caller names its own (calls on different streams run at the same time).
@@ -286,85 +286,130 @@ struct LookupState;       // lookup_host.inl
 struct SearchState;       // search_host.inl
 struct ComplianceTable;   // compliance_host.inl
 
+// The one owner of a CUDA event, destroyed with it (the counterpart of DevBuf)
+struct Event {
+    cudaEvent_t e = nullptr;
+    Event() = default;
+    Event(Event &&o) noexcept : e(o.e) { o.e = nullptr; }
+    Event &operator=(Event &&o) noexcept { std::swap(e, o.e); return *this; }
+    ~Event() { if (e) cudaEventDestroy(e); }
+    int create(unsigned flags) { CUDA_TRY(cudaEventCreateWithFlags(&e, flags)); return ABB_OK; }
+    operator cudaEvent_t() const { return e; }
+};
+
+// One global-bitmap walk tier: per-warp slots, each a visited bitmap over all nodes and a bounded queue with parents and depths.
+// alloc: `n_slots` slots of `words` bitmap words and `queue_cap` queue entries each, bitmaps cleared.
+struct GlobalSlots {
+    DevBuf bitmap, queue, par, dep;
+    int slots = 0; int64_t qcap = 0;
+    int alloc(int n_slots, int64_t words, int64_t queue_cap) {
+        slots = n_slots; qcap = queue_cap;
+        const size_t sl = static_cast<size_t>(slots);
+        int rc = ABB_OK;
+        ENS(bitmap, sl * words * 4); ENS(queue, sl * qcap * 4); ENS(par, sl * qcap * 4); ENS(dep, sl * qcap * 4);
+        if (rc) return rc;
+        CUDA_TRY(cudaMemset(bitmap.p, 0, sl * words * 4));
+        return ABB_OK;
+    }
+    void wire(WalkArgs &A, int64_t words) const {
+        A.g_bitmap = bitmap.as<uint32_t>(); A.g_queue = queue.as<int32_t>(); A.g_par = par.as<int32_t>(); A.g_dep = dep.as<int32_t>();
+        A.g_words = words; A.g_qcap = qcap;
+    }
+};
+
+// Everything the storage tiers of a walk need (enqueue_tiers)
+struct WalkTiers {
+    // tier bookkeeping: CTL_WORDS counters; the hand-off lists of S1 (two-ended), the mid tier, the big tier and G1
+    DevBuf ctl, ov[4];
+    // block tiers (walkb.cuh): mid = 8 warps, queue + table in shared memory; big = 32 warps, 192 KB table, queue in a global scratch slot per block
+    int block_tiers = 2;              // bit 0: mid tier (off by default: measured no faster than G1), bit 1: big tier (ABB_BLOCK_TIERS / abb_graph_set_option)
+    int mid_slots = 8192, mid_qcap = 4096, big_slots = 49152, big_qcap = 36864;
+    int big_grid = 0, mid_warps = 8;  // ABB_MID_WARPS=4: 4-warp mid blocks
+    int64_t big_limit = 0;            // the big tier takes S1's heavy hand-offs when there are at most this many (default 24 per SM)
+    DevBuf b_gq, b_gpar, b_gdep;
+    // tier G1: many per-warp slots (bitmap over all nodes + a bounded queue); tier GX: a few slots that can hold a whole-graph walk
+    GlobalSlots g1, gx; int64_t g_words = 0;
+    int s1_minb = 5;
+    int slice_align = 0;        // set while a host-mapped arena is the walk target
+    bool align_direct = true;
+};
+
+// root-frontier de-duplication workspace
+struct DedupWorkspace {
+    DevBuf sig, ssig, q, sq, head, gid, hp, glen, goff, arena, memoff, memsrc, memstate, indiv, cnt, tmp;
+    DevBuf gstart, gcount, gmaxd, gflags, ghist, lkey, lkey2, lgid, order;
+    bool enabled = true;
+    bool locality_order = true;   // walk the frontier groups in first-seed order (ABB_LOCALITY=0 disables)
+    bool last_walk = false;       // the last walk was de-duplicated
+};
+
+// host-API staging of one walk
+struct WalkStaging {
+    DevBuf roots, root_off, targets, qstart, qcount, qmaxd, qflags, qestart, qecount, qhist;
+    DevBuf nodes, parent, depth, edges, totals, hist_info_dev, hist_packed;
+    unsigned long long hist_info[2] = {0, 0};   // column mask, largest count of the walk just staged
+    bool hist_info_valid = false;
+    bool hist_pack = true;      // host results carry only the non-zero histogram columns at the narrowest width (histpack.cuh)
+    bool zero_copy = true;      // host-API walks write the node arena straight into pinned host memory when its size is known
+    int64_t hint_nodes = 0, hint_edges = 0, hint_nq = 0, hint_last_nodes = 0;
+    // size hint of the last PLAIN host walk (single roots, no parents / depths / edges), per spec: what the chunked path sizes its arenas from
+    abb_walk_spec plain_spec{};
+    int64_t plain_nq = -1, plain_nodes = 0;
+    int64_t last_walk_queries = 0;
+    Event ev_copy, ev_start, ev_end; bool timed = false;   // result copies wait for ev_copy; ev_start .. ev_end time the last walk
+};
+
+// chunked host walks (walk_host_chunked): a large plain batch is walked in `chunks` consecutive source ranges; each range's node arena
+// is DMA-copied to the host while the next range is walked (two device arenas, ping-pong)
+struct ChunkedWalk {
+    int chunks = 8;                  // ABB_CHUNKS / option "chunks"; applies to batches of >= chunk_min queries (measured at L: 1 piece 43.9 ms, 4: 42.4, 8: 40.6)
+    int64_t chunk_min = 2 << 20;
+    DevBuf nodes_alt, roots, sig, key, key2, idx, order, counts, tmp, qstart, qcount, qmaxd, qflags, qhist;
+    Event ev_walked, ev_copied[2];
+    std::vector<int64_t> hint; int64_t hint_nq = -1;   // nodes each chunk produced last time (same batch size / chunk count)
+    int last_host_chunks = 1;        // how many ranges the last host-buffer walk was split into (get_option "last_host_chunks")
+};
+
+// graph-constant tables of the exposure paths, built on first use (ensure_exposure_tables)
+struct ExposureTables {
+    // server tables: fan-out, and the principal rows each server contributes to a template
+    DevBuf srv_cred, srv_tool, srv_roff, srv_row, srv_rel;
+    // exposure tables: links of every finding node, templates of every vulnerable source, rows per finding node
+    DevBuf vs, loff, link, rows, toff, trow, trel, overflow;
+};
+
+// exposure-path per-call workspace
+struct PathsWorkspace {
+    DevBuf findings, f_off, scan_tmp;
+    // rows and links per finding; the host result's batch links and templates
+    DevBuf f_cnt, f_link, f_lcnt, link_off, link_vs, link_rel, link_roff, link_toff, need, ulist, nu, t_cnt, t_off, t_off_node, t_row, t_rel;
+    PathsArgs args{}; bool args_valid = false;   // the count pass's arguments, for the fill pass
+    int replicate_grid = 0, rank_keys_grid = 0;   // grids of the row-parallel kernels (row_grid)
+    Event ev_start, ev_end; bool timed = false;   // time the last count + fill
+};
+
+// finding-context workspace (context.cuh): per-finding bucket counts, totals, start offsets, source lists; the context kernels run on
+// paths_stream next to the impact walk (staged: the findings are on the device), ev time the count and fill passes
+struct ContextWorkspace {
+    DevBuf bcnt, cnt, start, src;
+    Event staged, ev[4];
+};
+
 struct abb_graph {
     int device = 0;
     GraphView v{};
     int64_t bytes = 0;
     int sm_count = 132;               // H100 SXM; set from the device in graph_finish_init
-    mutable std::mutex mu;            // serialises use of the shared workspace and of the snapshot tables
+    mutable std::mutex mu;            // serialises use of the workspaces and of the snapshot tables
     cudaStream_t stream = nullptr;    // host-API stream
     cudaStream_t copy_stream = nullptr;   // result copies that may overlap later kernels of the same call
     cudaStream_t paths_stream = nullptr;  // exposure-path pipeline of abb_exposure_host, run next to the walk
-    cudaEvent_t ev_copy = nullptr;
-    cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
-    bool walk_timed = false, paths_timed = false;
-    // tier bookkeeping
-    DevBuf ctl, ov1, ov2, ov3, ov4;
-    // block tiers (walkb.cuh): mid = 8 warps, queue + table in shared memory; big = 32 warps, 192 KB table, queue in a global scratch slot per block
-    int block_tiers = 2;              // bit 0: mid tier (off by default: measured no faster than G1), bit 1: big tier (ABB_BLOCK_TIERS / abb_graph_set_option)
-    int mid_slots = 8192, mid_qcap = 4096, big_slots = 49152, big_qcap = 36864;
-    int big_grid = 0;
-    int mid_warps = 8;                // ABB_MID_WARPS=4: 4-warp mid blocks
-    int64_t big_limit = 0;            // the big tier takes S1's heavy hand-offs when there are at most this many (default 24 per SM)
     int64_t nx_batch = 0;             // cap on betweenness sources per batch and on path-search slots (0: sized from free memory)
-    DevBuf b_gq, b_gpar, b_gdep;
-    // tier G1: many per-warp slots (bitmap over all nodes + a bounded queue); tier GX: a few slots that can hold a whole-graph walk
-    DevBuf g_bitmap, g_queue, g_par, g_dep;
-    int g_slots = 0; int64_t g_words = 0, g_qcap = 0;
-    DevBuf x_bitmap, x_queue, x_par, x_dep;
-    int x_slots = 0; int64_t x_qcap = 0;
-    // root-frontier de-duplication workspace
-    DevBuf dd_sig, dd_ssig, dd_q, dd_sq, dd_head, dd_gid, dd_hp, dd_glen, dd_goff, dd_arena, dd_memoff, dd_memsrc, dd_memstate, dd_indiv, dd_cnt, dd_tmp;
-    DevBuf dd_gstart, dd_gcount, dd_gmaxd, dd_gflags, dd_ghist, dd_lkey, dd_lkey2, dd_lgid, dd_order;
-    bool locality_order = true;   // walk the frontier groups in first-seed order (ABB_LOCALITY=0 disables)
-    bool dedup_enabled = true;
-    int slice_align = 0;        // set while a host-mapped arena is the walk target
-    bool align_direct = true;
-    bool hist_pack = true;      // host results carry only the non-zero histogram columns at the narrowest width (histpack.cuh)
-    DevBuf d_histinfo, d_hist_packed;
-    unsigned long long hist_info[2] = {0, 0};   // column mask, largest count of the walk just staged
-    bool hist_info_valid = false;
-    // chunked host walks (walk_host_chunked): a large plain batch is walked in `chunks` consecutive source ranges; each range's node arena
-    // is DMA-copied to the host while the next range is walked (two device arenas, ping-pong)
-    int chunks = 8;                  // ABB_CHUNKS / option "chunks"; applies to batches of >= chunk_min queries (measured at L: 1 piece 43.9 ms, 4: 42.4, 8: 40.6)
-    int64_t chunk_min = 2 << 20;
-    DevBuf d_nodes_alt, ck_roots, ck_sig, ck_key, ck_key2, ck_idx, ck_order, ck_counts, ck_tmp, ck_qstart, ck_qcount, ck_qmaxd, ck_qflags, ck_qhist;
-    cudaEvent_t ev_chunk_walked = nullptr, ev_chunk_copied[2] = {nullptr, nullptr};
-    std::vector<int64_t> chunk_hint;   // nodes each chunk produced last time (same batch size / chunk count)
-    int64_t chunk_hint_nq = -1;
-    // size hint of the last PLAIN host walk (single roots, no parents / depths / edges), per spec: what the chunked path sizes its arenas from
-    abb_walk_spec plain_spec{};
-    int64_t plain_nq = -1, plain_nodes = 0;
-    int last_host_chunks = 1;        // how many ranges the last host-buffer walk was split into (get_option "last_host_chunks")
-    bool zero_copy = true;      // host-API walks write the node arena straight into pinned host memory when its size is known
-    int64_t last_walk_queries = 0;
-    bool last_walk_dedup = false;
-    int s1_minb = 5;
     DevBuf identity_rank;
-    // host-API staging
-    DevBuf d_roots, d_root_off, d_targets, d_qstart, d_qcount, d_qmaxd, d_qflags, d_qestart, d_qecount, d_qhist;
-    DevBuf d_nodes, d_parent, d_depth, d_edges, d_totals;
-    int64_t hint_nodes = 0, hint_edges = 0, hint_nq = 0, hint_last_nodes = 0;
-    // graph-constant server tables (built on first use): fan-out, and the principal rows each server contributes to a template
-    DevBuf srv_cred, srv_tool, srv_roff, srv_row, srv_rel;
-    bool srv_table_ready = false;
-    // graph-constant exposure tables (built on first use, ensure_exposure_tables): links of every finding node, templates of every
-    // vulnerable source, rows per finding node
-    DevBuf x_vs, x_loff, x_link, x_rows, x_toff, x_trow, x_trel, x_overflow;
-    bool x_tables_ready = false;
-    // paths staging
-    DevBuf p_findings, p_off, p_scan_tmp;
-    // exposure-path per-call workspace: rows and links per finding; the host result's batch links and templates
-    DevBuf pl_cnt, pl_link, pl_lcnt, pl_off, pl_vs, pl_rel, pl_roff, pl_toff, pl_need, pl_ulist, pl_nu, pt_cnt, pt_off, pt_off_node, pt_row, pt_rel;
-    PathsArgs paths_args{};
-    bool paths_args_valid = false;
-    int replicate_grid = 0, rank_keys_grid = 0;   // grids of the row-parallel kernels (row_grid)
-    int64_t hint_rows = 0;
-    // finding-context workspace (context.cuh): per-finding bucket counts, totals, start offsets, source lists; the context kernels run on
-    // paths_stream next to the impact walk (cx_staged: the findings are on the device), cx_ev time the count and fill passes
-    DevBuf cx_bcnt, cx_cnt, cx_start, cx_src;
-    cudaEvent_t cx_staged = nullptr;
-    cudaEvent_t cx_ev[4] = {nullptr, nullptr, nullptr, nullptr};
+    // the walk's workspaces, then the path pipeline's and the finding context's (abb_exposure_host: who may use which, and when)
+    WalkTiers tiers; DedupWorkspace dedup; WalkStaging staging; ChunkedWalk chunked;
+    std::unique_ptr<ExposureTables> exposure;     // null: not built
+    PathsWorkspace paths; ContextWorkspace context;
     // snapshot tables, one owner per feature, each type declared in its *_host.inl.  A null table is not built; a rebuild drops the old
     // table, builds a new one aside and installs it only once every step has succeeded.  Read and replaced under mu.
     std::unique_ptr<ClusterTable> clusters;
@@ -392,51 +437,33 @@ static int graph_finish_init(abb_graph *g) {
     CUDA_TRY(cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking));
     CUDA_TRY(cudaStreamCreateWithFlags(&g->copy_stream, cudaStreamNonBlocking));
     CUDA_TRY(cudaStreamCreateWithFlags(&g->paths_stream, cudaStreamNonBlocking));
-    CUDA_TRY(cudaEventCreateWithFlags(&g->ev_copy, cudaEventDisableTiming));
-    CUDA_TRY(cudaEventCreateWithFlags(&g->ev_chunk_walked, cudaEventDisableTiming));
-    for (auto &e : g->ev_chunk_copied) CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    for (auto &e : g->ev) CUDA_TRY(cudaEventCreate(&e));
-    CUDA_TRY(cudaEventCreateWithFlags(&g->cx_staged, cudaEventDisableTiming));
-    for (auto &e : g->cx_ev) CUDA_TRY(cudaEventCreate(&e));
-    if (int rc = g->ctl.ensure(CTL_WORDS * sizeof(unsigned long long))) return rc;
+    for (Event *e : {&g->staging.ev_copy, &g->chunked.ev_walked, &g->chunked.ev_copied[0], &g->chunked.ev_copied[1], &g->context.staged})
+        if (int rc = e->create(cudaEventDisableTiming)) return rc;
+    for (Event *e : {&g->staging.ev_start, &g->staging.ev_end, &g->paths.ev_start, &g->paths.ev_end, &g->context.ev[0], &g->context.ev[1], &g->context.ev[2], &g->context.ev[3]})
+        if (int rc = e->create(cudaEventDefault)) return rc;
+    WalkTiers &wt = g->tiers;
+    if (int rc = wt.ctl.ensure(CTL_WORDS * sizeof(unsigned long long))) return rc;
     const int64_t n = g->v.n;
-    g->g_words = (n + 31) / 32 + 1;
+    wt.g_words = (n + 31) / 32 + 1;
     // tier G1: 40 warps per SM (latency-bound pointer chasing wants every warp it can get), queue bounded at 64K entries
-    g->g_qcap = std::min<int64_t>(n + 4096, 1 << 16);
-    g->g_slots = g->sm_count * 40;
-    if (const char *e = getenv("ABB_G1_WARPS_PER_SM")) g->g_slots = g->sm_count * std::max(4, std::min(48, atoi(e)));
-    {
-        const size_t sl = static_cast<size_t>(g->g_slots);
-        if (int rc = g->g_bitmap.ensure(sl * g->g_words * 4)) return rc;
-        if (int rc = g->g_queue.ensure(sl * g->g_qcap * 4)) return rc;
-        if (int rc = g->g_par.ensure(sl * g->g_qcap * 4)) return rc;
-        if (int rc = g->g_dep.ensure(sl * g->g_qcap * 4)) return rc;
-        CUDA_TRY(cudaMemset(g->g_bitmap.p, 0, sl * g->g_words * 4));
-    }
+    int g1_slots = g->sm_count * 40;
+    if (const char *e = getenv("ABB_G1_WARPS_PER_SM")) g1_slots = g->sm_count * std::max(4, std::min(48, atoi(e)));
+    if (int rc = wt.g1.alloc(g1_slots, wt.g_words, std::min<int64_t>(n + 4096, 1 << 16))) return rc;
     // tier GX: 8 slots that can hold any walk (every node once + re-seeded roots)
-    g->x_qcap = n + 4096;
-    g->x_slots = 8;
-    {
-        const size_t sl = static_cast<size_t>(g->x_slots);
-        if (int rc = g->x_bitmap.ensure(sl * g->g_words * 4)) return rc;
-        if (int rc = g->x_queue.ensure(sl * g->x_qcap * 4)) return rc;
-        if (int rc = g->x_par.ensure(sl * g->x_qcap * 4)) return rc;
-        if (int rc = g->x_dep.ensure(sl * g->x_qcap * 4)) return rc;
-        CUDA_TRY(cudaMemset(g->x_bitmap.p, 0, sl * g->g_words * 4));
-    }
-    if (const char *e = getenv("ABB_DEDUP")) g->dedup_enabled = atoi(e) != 0;
-    if (const char *e = getenv("ABB_BLOCK_TIERS")) g->block_tiers = atoi(e) & 3;
-    if (const char *e = getenv("ABB_LOCALITY")) g->locality_order = atoi(e) != 0;
-    g->big_grid = g->sm_count;
-    g->big_limit = 24ll * g->sm_count;
-    if (const char *e = getenv("ABB_BIG_LIMIT")) g->big_limit = atoll(e);
-    if (const char *e = getenv("ABB_MID_WARPS")) g->mid_warps = atoi(e) == 4 ? 4 : 8;
-    if (const char *e = getenv("ABB_S1_MINB")) g->s1_minb = atoi(e) == 4 ? 4 : 5;
-    if (const char *e = getenv("ABB_ZEROCOPY")) g->zero_copy = atoi(e) != 0;
-    if (const char *e = getenv("ABB_HIST_PACK")) g->hist_pack = atoi(e) != 0;
-    if (const char *e = getenv("ABB_CHUNKS")) g->chunks = std::max(1, std::min(64, atoi(e)));
-    if (const char *e = getenv("ABB_CHUNK_MIN")) g->chunk_min = std::max<int64_t>(2, atoll(e));
-    if (const char *e = getenv("ABB_ALIGN_DIRECT")) g->align_direct = atoi(e) != 0;
+    if (int rc = wt.gx.alloc(8, wt.g_words, n + 4096)) return rc;
+    if (const char *e = getenv("ABB_DEDUP")) g->dedup.enabled = atoi(e) != 0;
+    if (const char *e = getenv("ABB_BLOCK_TIERS")) wt.block_tiers = atoi(e) & 3;
+    if (const char *e = getenv("ABB_LOCALITY")) g->dedup.locality_order = atoi(e) != 0;
+    wt.big_grid = g->sm_count;
+    wt.big_limit = 24ll * g->sm_count;
+    if (const char *e = getenv("ABB_BIG_LIMIT")) wt.big_limit = atoll(e);
+    if (const char *e = getenv("ABB_MID_WARPS")) wt.mid_warps = atoi(e) == 4 ? 4 : 8;
+    if (const char *e = getenv("ABB_S1_MINB")) wt.s1_minb = atoi(e) == 4 ? 4 : 5;
+    if (const char *e = getenv("ABB_ZEROCOPY")) g->staging.zero_copy = atoi(e) != 0;
+    if (const char *e = getenv("ABB_HIST_PACK")) g->staging.hist_pack = atoi(e) != 0;
+    if (const char *e = getenv("ABB_CHUNKS")) g->chunked.chunks = std::max(1, std::min(64, atoi(e)));
+    if (const char *e = getenv("ABB_CHUNK_MIN")) g->chunked.chunk_min = std::max<int64_t>(2, atoll(e));
+    if (const char *e = getenv("ABB_ALIGN_DIRECT")) wt.align_direct = atoi(e) != 0;
     if (!g->v.rank) {
         if (int rc = g->identity_rank.ensure(static_cast<size_t>(n + 1) * 4)) return rc;
         std::vector<int32_t> id(static_cast<size_t>(n));
@@ -520,62 +547,60 @@ extern "C" int64_t abb_graph_bytes(const abb_graph *g) { return g ? g->bytes : 0
 extern "C" int abb_graph_set_dedup(abb_graph *g, int enabled) {
     if (!g) return fail(ABB_ERR_ARG, "null graph");
     std::lock_guard<std::mutex> lk(g->mu);
-    g->dedup_enabled = enabled != 0;
+    g->dedup.enabled = enabled != 0;
     return ABB_OK;
 }
 extern "C" int abb_graph_device(const abb_graph *g) { return g ? g->device : -1; }
 
+// The member behind one option, whatever its type: a flag stores value != 0, an int stores value & mask
+struct OptionRef {
+    bool *flag = nullptr; int *i32 = nullptr; int64_t *i64 = nullptr; int mask = -1;
+    OptionRef(bool &m) : flag(&m) {}
+    OptionRef(int &m, int mask_ = -1) : i32(&m), mask(mask_) {}
+    OptionRef(int64_t &m) : i64(&m) {}
+    int64_t get() const { return flag ? *flag : i32 ? *i32 : *i64; }
+    void set(int64_t value) const { if (flag) *flag = value != 0; else if (i32) *i32 = static_cast<int>(value) & mask; else *i64 = value; }
+};
+
 // Tuning / test switches of a graph handle.  Results never depend on them (every tier is bit-identical; the GPU tests
 // run the suite with the block tiers on, off and shrunk so that every hand-off between tiers is exercised).
+// set_option accepts values in [lo, hi] and otherwise fails with `range`; a null `range` marks a read-only option.
+static const struct GraphOption {
+    const char *name; OptionRef (*member)(abb_graph &g); int64_t lo, hi; const char *range;
+} g_options[] = {
+    {"dedup", [](abb_graph &g) { return OptionRef(g.dedup.enabled); }, INT64_MIN, INT64_MAX, ""},
+    {"block_tiers", [](abb_graph &g) { return OptionRef(g.tiers.block_tiers, 3); }, INT64_MIN, INT64_MAX, ""},
+    {"mid_qcap", [](abb_graph &g) { return OptionRef(g.tiers.mid_qcap); }, 32, 4096, "mid_qcap must be in [32, 4096]"},
+    {"big_qcap", [](abb_graph &g) { return OptionRef(g.tiers.big_qcap); }, 32, 36864, "big_qcap must be in [32, 36864]"},
+    {"zero_copy", [](abb_graph &g) { return OptionRef(g.staging.zero_copy); }, INT64_MIN, INT64_MAX, ""},
+    {"hist_pack", [](abb_graph &g) { return OptionRef(g.staging.hist_pack); }, INT64_MIN, INT64_MAX, ""},
+    {"chunks", [](abb_graph &g) { return OptionRef(g.chunked.chunks); }, 1, 64, "chunks must be in [1, 64]"},
+    {"chunk_min", [](abb_graph &g) { return OptionRef(g.chunked.chunk_min); }, 2, INT64_MAX, "chunk_min must be >= 2"},
+    {"last_host_chunks", [](abb_graph &g) { return OptionRef(g.chunked.last_host_chunks); }, 0, 0, nullptr},
+    {"big_limit", [](abb_graph &g) { return OptionRef(g.tiers.big_limit); }, 0, INT64_MAX, "big_limit must be >= 0"},
+    {"nx_batch", [](abb_graph &g) { return OptionRef(g.nx_batch); }, 0, INT64_MAX, "nx_batch must be >= 0"},
+    {"delta_union_limit", [](abb_graph &g) { return OptionRef(g.dl_union_limit); }, 0, DL_UNION_LIMIT, "delta_union_limit must be in [0, 2^27]"},
+};
+
+static const GraphOption *find_option(const char *name) {
+    for (const GraphOption &o : g_options) if (strcmp(o.name, name) == 0) return &o;
+    return nullptr;
+}
+
 extern "C" int abb_graph_set_option(abb_graph *g, const char *name, int64_t value) {
     if (!g || !name) return fail(ABB_ERR_ARG, "null argument");
     std::lock_guard<std::mutex> lk(g->mu);
-    const std::string k(name);
-    if (k == "dedup") g->dedup_enabled = value != 0;
-    else if (k == "block_tiers") g->block_tiers = static_cast<int>(value) & 3;
-    else if (k == "mid_qcap") {
-        if (value < 32 || value > 4096) return fail(ABB_ERR_ARG, "mid_qcap must be in [32, 4096]");
-        g->mid_qcap = static_cast<int>(value);
-    } else if (k == "big_qcap") {
-        if (value < 32 || value > 36864) return fail(ABB_ERR_ARG, "big_qcap must be in [32, 36864]");
-        g->big_qcap = static_cast<int>(value);
-    } else if (k == "zero_copy") g->zero_copy = value != 0;
-    else if (k == "hist_pack") g->hist_pack = value != 0;
-    else if (k == "chunks") {
-        if (value < 1 || value > 64) return fail(ABB_ERR_ARG, "chunks must be in [1, 64]");
-        g->chunks = static_cast<int>(value);
-    } else if (k == "chunk_min") {
-        if (value < 2) return fail(ABB_ERR_ARG, "chunk_min must be >= 2");
-        g->chunk_min = value;
-    }
-    else if (k == "big_limit") {
-        if (value < 0) return fail(ABB_ERR_ARG, "big_limit must be >= 0");
-        g->big_limit = value;
-    } else if (k == "nx_batch") {
-        if (value < 0) return fail(ABB_ERR_ARG, "nx_batch must be >= 0");
-        g->nx_batch = value;
-    } else if (k == "delta_union_limit") {
-        if (value < 0 || value > DL_UNION_LIMIT) return fail(ABB_ERR_ARG, "delta_union_limit must be in [0, 2^27]");
-        g->dl_union_limit = value;
-    } else return fail(ABB_ERR_ARG, "unknown option '%s'", name);
+    const GraphOption *o = find_option(name);
+    if (!o || !o->range) return fail(ABB_ERR_ARG, "unknown option '%s'", name);
+    if (value < o->lo || value > o->hi) return fail(ABB_ERR_ARG, "%s", o->range);
+    o->member(*g).set(value);
     return ABB_OK;
 }
 extern "C" int64_t abb_graph_get_option(const abb_graph *g, const char *name) {
     if (!g || !name) return -1;
-    const std::string k(name);
-    if (k == "dedup") return g->dedup_enabled;
-    if (k == "block_tiers") return g->block_tiers;
-    if (k == "mid_qcap") return g->mid_qcap;
-    if (k == "big_qcap") return g->big_qcap;
-    if (k == "zero_copy") return g->zero_copy;
-    if (k == "hist_pack") return g->hist_pack;
-    if (k == "chunks") return g->chunks;
-    if (k == "chunk_min") return g->chunk_min;
-    if (k == "last_host_chunks") return g->last_host_chunks;
-    if (k == "big_limit") return g->big_limit;
-    if (k == "nx_batch") return g->nx_batch;
-    if (k == "delta_union_limit") return g->dl_union_limit;
-    return -1;
+    std::lock_guard<std::mutex> lk(g->mu);
+    const GraphOption *o = find_option(name);
+    return o ? o->member(const_cast<abb_graph &>(*g)).get() : -1;   // only read
 }
 
 extern "C" void abb_graph_free(abb_graph *g) {
@@ -661,7 +686,7 @@ static int launch_smem(const abb_graph *g, const WalkArgs &A, int64_t max_items,
 template <int H, int Q, int WARPS>
 static int launch_smem_variant(const abb_graph *g, const WalkArgs &A, int64_t max_items, bool par, bool meta, bool bud, cudaStream_t st) {
     // MINB: resident blocks the register allocation aims for — 5 (48 registers, 40 warps/SM) or 4 (64 registers, 32 warps/SM; ABB_S1_MINB=4)
-#define V(P, M, B) if (par == P && meta == M && bud == B) return g->s1_minb == 4 ? launch_smem<H, Q, WARPS, P, M, B, 4>(g, A, max_items, st) : launch_smem<H, Q, WARPS, P, M, B, 5>(g, A, max_items, st)
+#define V(P, M, B) if (par == P && meta == M && bud == B) return g->tiers.s1_minb == 4 ? launch_smem<H, Q, WARPS, P, M, B, 4>(g, A, max_items, st) : launch_smem<H, Q, WARPS, P, M, B, 5>(g, A, max_items, st)
     V(false, false, false); V(false, false, true); V(false, true, false); V(false, true, true);
     V(true, false, false); V(true, false, true); V(true, true, false); V(true, true, true);
 #undef V
@@ -722,9 +747,10 @@ static int enqueue_tiers(abb_graph *g, WalkArgs A, int64_t max_items, unsigned l
     const bool par = fl & ABB_WALK_PARENTS;
     const bool meta = A.spec.rel_mask != 0xFFFFFFFFu || (fl & ABB_WALK_TRAVERSABLE_ONLY);
     const bool bud = A.spec.max_nodes >= 0 || A.spec.max_edges >= 0;
-    int32_t *ovs[4] = {g->ov1.as<int32_t>(), g->ov2.as<int32_t>(), g->ov3.as<int32_t>(), g->ov4.as<int32_t>()};
+    WalkTiers &wt = g->tiers;
+    int32_t *ovs[4] = {wt.ov[0].as<int32_t>(), wt.ov[1].as<int32_t>(), wt.ov[2].as<int32_t>(), wt.ov[3].as<int32_t>()};
     A.list_cap = max_items;
-    A.slice_align = g->slice_align;
+    A.slice_align = wt.slice_align;
     // S1: two-ended hand-off list in ovs[0]
     A.ctl = ctl; A.overflow = ovs[0]; A.ov_cnt_front = ctl + 1; A.ov_cnt_back = ctl + 3;
     if (int rc = launch_smem_variant<S1_H, S1_Q, S1_WARPS>(g, A, max_items, par, meta, bud, st)) return rc;
@@ -732,18 +758,18 @@ static int enqueue_tiers(abb_graph *g, WalkArgs A, int64_t max_items, unsigned l
     const bool plain = !bud && !(fl & (ABB_WALK_TARGET | ABB_WALK_EDGES));
     bool front_taken = false;                       // S1's heavy part routed (to the big tier when few, else first in line for the warp tier)
     unsigned long long *to_big = ctl + CTL_ROUTE, *to_warp = ctl + CTL_ROUTE + 1;
-    if (plain && (g->block_tiers & 2) && idb <= 26) {
-        if (int rc = LAUNCH(route_heavy_kernel, 1, 1, 0, st, ctl + 1, to_big, to_warp, static_cast<unsigned long long>(g->big_limit))) return rc;
+    if (plain && (wt.block_tiers & 2) && idb <= 26) {
+        if (int rc = LAUNCH(route_heavy_kernel, 1, 1, 0, st, ctl + 1, to_big, to_warp, static_cast<unsigned long long>(wt.big_limit))) return rc;
         // big tier: the heavy (front) part of S1's list; what it cannot hold goes to a list of its own (ovs[2]) that the next tier
         // reads after S1's back part — NOT onto S1's list: front + back may already fill it
         A.qlist = ovs[0]; A.nq = 0; A.nq_dev = to_big; A.nq_back_dev = nullptr; A.ctl = ctl + 4 * 1;
         A.overflow = ovs[2]; A.ov_cnt_front = ctl + 4 * 1 + 1; A.ov_cnt_back = nullptr;
-        const size_t words = static_cast<size_t>(g->big_grid) * g->big_qcap;
-        if (int rc = g->b_gq.ensure(words * 4)) return rc;
-        if (par) if (int rc = g->b_gpar.ensure(words * 4)) return rc;
-        if (fl & ABB_WALK_DEPTHS) if (int rc = g->b_gdep.ensure(words * 4)) return rc;
-        BlockTier T{static_cast<uint32_t>(g->big_slots), g->big_qcap, idb, g->b_gq.as<int32_t>(), g->b_gpar.as<int32_t>(), g->b_gdep.as<int32_t>()};
-        int rc = meta ? launch_block<32, false, true, true, 1>(g, A, T, g->big_grid, st) : launch_block<32, false, true, false, 1>(g, A, T, g->big_grid, st);
+        const size_t words = static_cast<size_t>(wt.big_grid) * wt.big_qcap;
+        if (int rc = wt.b_gq.ensure(words * 4)) return rc;
+        if (par) if (int rc = wt.b_gpar.ensure(words * 4)) return rc;
+        if (fl & ABB_WALK_DEPTHS) if (int rc = wt.b_gdep.ensure(words * 4)) return rc;
+        BlockTier T{static_cast<uint32_t>(wt.big_slots), wt.big_qcap, idb, wt.b_gq.as<int32_t>(), wt.b_gpar.as<int32_t>(), wt.b_gdep.as<int32_t>()};
+        int rc = meta ? launch_block<32, false, true, true, 1>(g, A, T, wt.big_grid, st) : launch_block<32, false, true, false, 1>(g, A, T, wt.big_grid, st);
         if (rc) return rc;
         front_taken = true;
     }
@@ -752,13 +778,13 @@ static int enqueue_tiers(abb_graph *g, WalkArgs A, int64_t max_items, unsigned l
     int32_t *in_list = ovs[0];
     const int32_t *in_list2 = front_taken ? ovs[2] : nullptr;
     const unsigned long long *in_cnt2 = front_taken ? ctl + 4 * 1 + 1 : nullptr;
-    if (plain && (g->block_tiers & 1) && idb <= 28) {
+    if (plain && (wt.block_tiers & 1) && idb <= 28) {
         A.qlist = in_list; A.nq = 0; A.nq_dev = in_front; A.nq_back_dev = in_back; A.qlist2 = in_list2; A.nq2_dev = in_cnt2; A.ctl = ctl + 4 * 2;
         A.overflow = ovs[1]; A.ov_cnt_front = ctl + 4 * 2 + 1; A.ov_cnt_back = nullptr;
-        BlockTier T{static_cast<uint32_t>(g->mid_slots), g->mid_qcap, idb, nullptr, nullptr, nullptr};
+        BlockTier T{static_cast<uint32_t>(wt.mid_slots), wt.mid_qcap, idb, nullptr, nullptr, nullptr};
         int rc;
-        if (g->mid_warps == 4) {               // 4-warp blocks: half the table / queue, twice the walks in flight per SM
-            T.slots = static_cast<uint32_t>(std::min(g->mid_slots, 4096)); T.qcap = std::min(g->mid_qcap, 2048);
+        if (wt.mid_warps == 4) {               // 4-warp blocks: half the table / queue, twice the walks in flight per SM
+            T.slots = static_cast<uint32_t>(std::min(wt.mid_slots, 4096)); T.qcap = std::min(wt.mid_qcap, 2048);
             if (par && meta) rc = launch_block<4, true, true, true, 6>(g, A, T, 0, st);
             else if (par) rc = launch_block<4, true, true, false, 6>(g, A, T, 0, st);
             else if (meta) rc = launch_block<4, true, false, true, 8>(g, A, T, 0, st);
@@ -773,14 +799,12 @@ static int enqueue_tiers(abb_graph *g, WalkArgs A, int64_t max_items, unsigned l
     // G1
     A.qlist = in_list; A.nq = 0; A.nq_dev = in_front; A.nq_back_dev = in_back; A.qlist2 = in_list2; A.nq2_dev = in_cnt2; A.ctl = ctl + 4 * 3;
     A.overflow = ovs[3]; A.ov_cnt_front = ctl + 4 * 3 + 1; A.ov_cnt_back = nullptr;
-    A.g_bitmap = g->g_bitmap.as<uint32_t>(); A.g_queue = g->g_queue.as<int32_t>(); A.g_par = g->g_par.as<int32_t>(); A.g_dep = g->g_dep.as<int32_t>();
-    A.g_words = g->g_words; A.g_qcap = g->g_qcap;
-    if (int rc = launch_global_variant(A, g->g_slots, g->sm_count, meta, bud, st)) return rc;
+    wt.g1.wire(A, wt.g_words);
+    if (int rc = launch_global_variant(A, wt.g1.slots, g->sm_count, meta, bud, st)) return rc;
     // GX
     A.qlist = ovs[3]; A.nq_dev = ctl + 4 * 3 + 1; A.nq_back_dev = nullptr; A.qlist2 = nullptr; A.nq2_dev = nullptr; A.ctl = ctl + 4 * 4; A.overflow = nullptr; A.ov_cnt_front = A.ov_cnt_back = nullptr;
-    A.g_bitmap = g->x_bitmap.as<uint32_t>(); A.g_queue = g->x_queue.as<int32_t>(); A.g_par = g->x_par.as<int32_t>(); A.g_dep = g->x_dep.as<int32_t>();
-    A.g_qcap = g->x_qcap;
-    return launch_global_variant(A, g->x_slots, g->sm_count, meta, bud, st);
+    wt.gx.wire(A, wt.g_words);
+    return launch_global_variant(A, wt.gx.slots, g->sm_count, meta, bud, st);
 }
 
 static int check_walk_io(const abb_walk_spec *spec, const abb_walk_io *io) {
@@ -808,60 +832,61 @@ static int enqueue_dedup_walk(abb_graph *g, const abb_walk_spec *spec, const abb
     const size_t q1 = static_cast<size_t>(nq) + 2;
     const uint32_t fl = spec->flags;
     int rc = ABB_OK;
-    ENS(dd_sig, q1 * 8); ENS(dd_ssig, q1 * 8); ENS(dd_q, q1 * 4); ENS(dd_sq, q1 * 4); ENS(dd_head, q1); ENS(dd_gid, q1 * 8); ENS(dd_hp, q1 * 8);
-    ENS(dd_glen, q1 * 8); ENS(dd_goff, q1 * 8); ENS(dd_arena, q1 * 4 * L1_CAP); ENS(dd_memoff, q1 * 8); ENS(dd_memsrc, q1 * 4); ENS(dd_memstate, q1 * 4);
-    ENS(dd_indiv, q1 * 4); ENS(dd_cnt, 8 * sizeof(unsigned long long));
-    ENS(dd_lkey, q1 * 4); ENS(dd_lkey2, q1 * 4); ENS(dd_lgid, q1 * 4); ENS(dd_order, q1 * 4);
-    ENS(dd_gstart, q1 * 8); ENS(dd_gcount, q1 * 4); ENS(dd_gmaxd, q1 * 4); ENS(dd_gflags, q1 * 4);
-    if (fl & ABB_WALK_HIST) { ENS(dd_ghist, q1 * ABB_N_ENTITY_TYPES * 4); }
+    DedupWorkspace &D = g->dedup;
+    ENS(D.sig, q1 * 8); ENS(D.ssig, q1 * 8); ENS(D.q, q1 * 4); ENS(D.sq, q1 * 4); ENS(D.head, q1); ENS(D.gid, q1 * 8); ENS(D.hp, q1 * 8);
+    ENS(D.glen, q1 * 8); ENS(D.goff, q1 * 8); ENS(D.arena, q1 * 4 * L1_CAP); ENS(D.memoff, q1 * 8); ENS(D.memsrc, q1 * 4); ENS(D.memstate, q1 * 4);
+    ENS(D.indiv, q1 * 4); ENS(D.cnt, 8 * sizeof(unsigned long long));
+    ENS(D.lkey, q1 * 4); ENS(D.lkey2, q1 * 4); ENS(D.lgid, q1 * 4); ENS(D.order, q1 * 4);
+    ENS(D.gstart, q1 * 8); ENS(D.gcount, q1 * 4); ENS(D.gmaxd, q1 * 4); ENS(D.gflags, q1 * 4);
+    if (fl & ABB_WALK_HIST) { ENS(D.ghist, q1 * ABB_N_ENTITY_TYPES * 4); }
     if (rc) return rc;
-    unsigned long long *cnt = g->dd_cnt.as<unsigned long long>();
-    unsigned long long *sig = g->dd_sig.as<unsigned long long>(), *ssig = g->dd_ssig.as<unsigned long long>();
-    int32_t *qi = g->dd_q.as<int32_t>(), *sq = g->dd_sq.as<int32_t>(), *indiv = g->dd_indiv.as<int32_t>();
-    uint8_t *head = g->dd_head.as<uint8_t>();
-    int64_t *gid = g->dd_gid.as<int64_t>(), *hp = g->dd_hp.as<int64_t>(), *glen = g->dd_glen.as<int64_t>(), *goff = g->dd_goff.as<int64_t>();
-    int64_t *memoff = g->dd_memoff.as<int64_t>();
+    unsigned long long *cnt = D.cnt.as<unsigned long long>();
+    unsigned long long *sig = D.sig.as<unsigned long long>(), *ssig = D.ssig.as<unsigned long long>();
+    int32_t *qi = D.q.as<int32_t>(), *sq = D.sq.as<int32_t>(), *indiv = D.indiv.as<int32_t>();
+    uint8_t *head = D.head.as<uint8_t>();
+    int64_t *gid = D.gid.as<int64_t>(), *hp = D.hp.as<int64_t>(), *glen = D.glen.as<int64_t>(), *goff = D.goff.as<int64_t>();
+    int64_t *memoff = D.memoff.as<int64_t>();
     const unsigned blocks = static_cast<unsigned>((nq + 255) / 256);
     CUDA_TRY(cudaMemsetAsync(cnt, 0, 8 * sizeof(unsigned long long), st));
     CUDA_TRY(cudaMemsetAsync(glen, 0, q1 * 8, st));
     if ((rc = LAUNCH(dedup_sig_kernel, blocks, 256, 0, st, g->v, *spec, io->roots, nq, sig, qi))) return rc;
-    if ((rc = cub_run(g->dd_tmp, [&](void *t, size_t &b) { return cub::DeviceRadixSort::SortPairs(t, b, sig, ssig, qi, sq, static_cast<int>(nq), 0, SIG_BITS, st); })))
+    if ((rc = cub_run(D.tmp, [&](void *t, size_t &b) { return cub::DeviceRadixSort::SortPairs(t, b, sig, ssig, qi, sq, static_cast<int>(nq), 0, SIG_BITS, st); })))
         return rc;
     if ((rc = LAUNCH(dedup_heads_kernel, blocks, 256, 0, st, ssig, sq, nq, head, indiv, cnt))) return rc;
     cub::TransformInputIterator<int64_t, HeadToI64, const uint8_t *> head64(head, HeadToI64());
-    if ((rc = cub_run(g->dd_tmp, [&](void *t, size_t &b) { return cub::DeviceScan::InclusiveSum(t, b, head64, gid, static_cast<int>(nq), st); }))) return rc;
-    if ((rc = select_flagged(g->dd_tmp, head, hp, cnt, static_cast<int>(nq), st))) return rc;
+    if ((rc = cub_run(D.tmp, [&](void *t, size_t &b) { return cub::DeviceScan::InclusiveSum(t, b, head64, gid, static_cast<int>(nq), st); }))) return rc;
+    if ((rc = select_flagged(D.tmp, head, hp, cnt, static_cast<int>(nq), st))) return rc;
     if ((rc = LAUNCH(dedup_groups_kernel, static_cast<unsigned>((nq + 1 + 255) / 256), 256, 0, st, g->v, *spec, io->roots, sq, hp, cnt, glen, memoff))) return rc;
     // glen is passed non-const here, unlike scan_i64's input: a different cub instantiation
-    if ((rc = cub_run(g->dd_tmp, [&](void *t, size_t &b) { return cub::DeviceScan::ExclusiveSum(t, b, glen, goff, static_cast<int>(nq + 1), st); }))) return rc;
-    if ((rc = LAUNCH(dedup_roots_kernel, blocks, 256, 0, st, g->v, *spec, io->roots, sq, hp, cnt, goff, g->dd_arena.as<int32_t>()))) return rc;
-    if ((rc = LAUNCH(dedup_members_kernel, blocks, 256, 0, st, g->v, *spec, io->roots, sq, head, gid, goff, g->dd_arena.as<int32_t>(), g->dd_memsrc.as<int32_t>(),
-                     g->dd_memstate.as<int32_t>(), indiv, cnt)))
+    if ((rc = cub_run(D.tmp, [&](void *t, size_t &b) { return cub::DeviceScan::ExclusiveSum(t, b, glen, goff, static_cast<int>(nq + 1), st); }))) return rc;
+    if ((rc = LAUNCH(dedup_roots_kernel, blocks, 256, 0, st, g->v, *spec, io->roots, sq, hp, cnt, goff, D.arena.as<int32_t>()))) return rc;
+    if ((rc = LAUNCH(dedup_members_kernel, blocks, 256, 0, st, g->v, *spec, io->roots, sq, head, gid, goff, D.arena.as<int32_t>(), D.memsrc.as<int32_t>(),
+                     D.memstate.as<int32_t>(), indiv, cnt)))
         return rc;
-    unsigned long long *ctl = g->ctl.as<unsigned long long>();
+    unsigned long long *ctl = g->tiers.ctl.as<unsigned long long>();
     // canonical walks: one per group, seeded with the shared frontier, one level shallower, depths biased by one
     WalkArgs C{};
     C.g = g->v; C.spec = *spec; C.io = *io;
     C.spec.max_depth = spec->max_depth < 0 ? -1 : spec->max_depth - 1;
     C.spec.flags = (fl & ~(ABB_WALK_OMIT_ROOTS | ABB_WALK_REAL_ROOTS)) | ABB_WALK_MARK_ROOTS;
-    C.io.roots = g->dd_arena.as<int32_t>(); C.io.root_off = goff;
-    C.io.q_start = g->dd_gstart.as<int64_t>(); C.io.q_count = g->dd_gcount.as<int32_t>(); C.io.q_maxd = g->dd_gmaxd.as<int32_t>();
-    C.io.q_flags = g->dd_gflags.as<int32_t>(); C.io.q_hist = g->dd_ghist.as<uint32_t>();
+    C.io.roots = D.arena.as<int32_t>(); C.io.root_off = goff;
+    C.io.q_start = D.gstart.as<int64_t>(); C.io.q_count = D.gcount.as<int32_t>(); C.io.q_maxd = D.gmaxd.as<int32_t>();
+    C.io.q_flags = D.gflags.as<int32_t>(); C.io.q_hist = D.ghist.as<uint32_t>();
     C.qlist = nullptr; C.nq = 0; C.nq_dev = cnt;
-    if (g->locality_order) {
+    if (D.locality_order) {
         // walk order = first-seed order (a 2 M-key radix sort over the node-id bits, ~0.1 ms): neighbouring groups share rows in L2
-        uint32_t *lkey = g->dd_lkey.as<uint32_t>(), *lkey2 = g->dd_lkey2.as<uint32_t>();
-        int32_t *lgid = g->dd_lgid.as<int32_t>(), *order = g->dd_order.as<int32_t>();
-        if ((rc = LAUNCH(dedup_locality_keys_kernel, blocks, 256, 0, st, cnt, goff, g->dd_arena.as<int32_t>(), lkey, lgid, nq))) return rc;
-        if ((rc = cub_run(g->dd_tmp, [&](void *t, size_t &b) { return cub::DeviceRadixSort::SortPairs(t, b, lkey, lkey2, lgid, order, static_cast<int>(nq), 0, 32, st); })))
+        uint32_t *lkey = D.lkey.as<uint32_t>(), *lkey2 = D.lkey2.as<uint32_t>();
+        int32_t *lgid = D.lgid.as<int32_t>(), *order = D.order.as<int32_t>();
+        if ((rc = LAUNCH(dedup_locality_keys_kernel, blocks, 256, 0, st, cnt, goff, D.arena.as<int32_t>(), lkey, lgid, nq))) return rc;
+        if ((rc = cub_run(D.tmp, [&](void *t, size_t &b) { return cub::DeviceRadixSort::SortPairs(t, b, lkey, lkey2, lgid, order, static_cast<int>(nq), 0, 32, st); })))
             return rc;
         C.qlist = order;
     }
     C.depth_bias = 1; C.hist_roots = 1;
-    C.mem_off = memoff; C.mem_src = g->dd_memsrc.as<int32_t>(); C.mem_state = g->dd_memstate.as<int32_t>();
+    C.mem_off = memoff; C.mem_src = D.memsrc.as<int32_t>(); C.mem_state = D.memstate.as<int32_t>();
     if ((rc = enqueue_tiers(g, C, nq, ctl, st))) return rc;
     if ((rc = LAUNCH(dedup_share_kernel, grid_for(nq, 256, g->sm_count, 8), 256, 0, st,
-                     sq, gid, g->dd_memstate.as<int32_t>(), cnt, C.io.q_start, C.io.q_count, C.io.q_maxd, C.io.q_flags, C.io.q_hist, io->q_start, io->q_count,
+                     sq, gid, D.memstate.as<int32_t>(), cnt, C.io.q_start, C.io.q_count, C.io.q_maxd, C.io.q_flags, C.io.q_hist, io->q_start, io->q_count,
                      io->q_maxd, io->q_flags, (fl & ABB_WALK_HIST) ? io->q_hist : nullptr, indiv, cnt)))
         return rc;
     // individual walks: ineligible sources, signature collisions, sources reached by their own group's walk
@@ -873,7 +898,7 @@ static int enqueue_dedup_walk(abb_graph *g, const abb_walk_spec *spec, const abb
 
 static bool dedup_applies(const abb_graph *g, const abb_walk_spec *spec, const abb_walk_io *io) {
     const uint32_t fl = spec->flags;
-    return g->dedup_enabled && !io->root_off && io->n_queries >= 256 && (fl & ABB_WALK_MARK_ROOTS) && (fl & ABB_WALK_OMIT_ROOTS) &&
+    return g->dedup.enabled && !io->root_off && io->n_queries >= 256 && (fl & ABB_WALK_MARK_ROOTS) && (fl & ABB_WALK_OMIT_ROOTS) &&
            !(fl & (ABB_WALK_TARGET | ABB_WALK_EDGES | ABB_WALK_PARENTS)) && spec->max_nodes < 0 && spec->max_edges < 0 && spec->max_depth != 0;
 }
 
@@ -881,18 +906,15 @@ static int enqueue_walk(abb_graph *g, const abb_walk_spec *spec, const abb_walk_
     if (int rc = check_walk_io(spec, io)) return rc;
     CUDA_TRY(cudaMemsetAsync(io->totals, 0, 2 * sizeof(unsigned long long), st));
     if (io->n_queries == 0) return ABB_OK;
-    if (int rc = g->ov1.ensure(static_cast<size_t>(io->n_queries) * 4)) return rc;
-    if (int rc = g->ov2.ensure(static_cast<size_t>(io->n_queries) * 4)) return rc;
-    if (int rc = g->ov3.ensure(static_cast<size_t>(io->n_queries) * 4)) return rc;
-    if (int rc = g->ov4.ensure(static_cast<size_t>(io->n_queries) * 4)) return rc;
-    CUDA_TRY(cudaMemsetAsync(g->ctl.p, 0, CTL_WORDS * sizeof(unsigned long long), st));
-    g->last_walk_queries = io->n_queries;
-    g->last_walk_dedup = dedup_applies(g, spec, io);
-    if (g->last_walk_dedup) return enqueue_dedup_walk(g, spec, io, st);
+    for (DevBuf &ov : g->tiers.ov) if (int rc = ov.ensure(static_cast<size_t>(io->n_queries) * 4)) return rc;
+    CUDA_TRY(cudaMemsetAsync(g->tiers.ctl.p, 0, CTL_WORDS * sizeof(unsigned long long), st));
+    g->staging.last_walk_queries = io->n_queries;
+    g->dedup.last_walk = dedup_applies(g, spec, io);
+    if (g->dedup.last_walk) return enqueue_dedup_walk(g, spec, io, st);
     WalkArgs A{};
     A.g = g->v; A.spec = *spec; A.io = *io;
     A.qlist = nullptr; A.nq = io->n_queries; A.nq_dev = nullptr;
-    return enqueue_tiers(g, A, io->n_queries, g->ctl.as<unsigned long long>(), st);
+    return enqueue_tiers(g, A, io->n_queries, g->tiers.ctl.as<unsigned long long>(), st);
 }
 
 extern "C" int abb_walk_launch(abb_graph *g, const abb_walk_spec *spec, const abb_walk_io *io, void *stream) {
@@ -901,11 +923,11 @@ extern "C" int abb_walk_launch(abb_graph *g, const abb_walk_spec *spec, const ab
     DeviceGuard dg(g->device);
     std::lock_guard<std::mutex> lk(g->mu);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    CUDA_TRY(cudaEventRecord(g->ev[0], st));
+    CUDA_TRY(cudaEventRecord(g->staging.ev_start, st));
     int rc = enqueue_walk(g, spec, io, st);
     if (rc) return rc;
-    CUDA_TRY(cudaEventRecord(g->ev[1], st));
-    g->walk_timed = true;
+    CUDA_TRY(cudaEventRecord(g->staging.ev_end, st));
+    g->staging.timed = true;
     return ABB_OK;
 }
 
@@ -917,21 +939,23 @@ extern "C" int abb_walk_signatures(abb_graph *g, const abb_walk_spec *spec, cons
 }
 
 extern "C" float abb_last_walk_ms(abb_graph *g) {
-    if (!g || !g->walk_timed) return -1.f;
+    if (!g) return -1.f;
     DeviceGuard dg(g->device);
+    std::lock_guard<std::mutex> lk(g->mu);   // both events of one call: another thread's call records them under the lock
+    if (!g->staging.timed) return -1.f;
     float ms = -1.f;
-    if (cudaEventSynchronize(g->ev[1]) != cudaSuccess) return -1.f;
-    if (cudaEventElapsedTime(&ms, g->ev[0], g->ev[1]) != cudaSuccess) return -1.f;
+    if (cudaEventSynchronize(g->staging.ev_end) != cudaSuccess) return -1.f;
+    if (cudaEventElapsedTime(&ms, g->staging.ev_start, g->staging.ev_end) != cudaSuccess) return -1.f;
     return ms;
 }
 extern "C" int abb_last_walk_stats(abb_graph *g, int64_t *out4) {
     if (!g || !out4) return fail(ABB_ERR_ARG, "null argument");
     DeviceGuard dg(g->device);
     std::lock_guard<std::mutex> lk(g->mu);
-    out4[0] = g->last_walk_queries; out4[1] = out4[2] = out4[3] = 0;
-    if (g->last_walk_dedup && g->dd_cnt.p) {
+    out4[0] = g->staging.last_walk_queries; out4[1] = out4[2] = out4[3] = 0;
+    if (g->dedup.last_walk && g->dedup.cnt.p) {
         unsigned long long c[3] = {0, 0, 0};
-        CUDA_TRY(cudaMemcpy(c, g->dd_cnt.p, sizeof c, cudaMemcpyDeviceToHost));
+        CUDA_TRY(cudaMemcpy(c, g->dedup.cnt.p, sizeof c, cudaMemcpyDeviceToHost));
         out4[1] = static_cast<int64_t>(c[0]); out4[2] = static_cast<int64_t>(c[1]); out4[3] = static_cast<int64_t>(c[2]);
     }
     return ABB_OK;
@@ -942,7 +966,7 @@ extern "C" int abb_last_walk_tier_counts(abb_graph *g, int64_t *out8) {
     DeviceGuard dg(g->device);
     std::lock_guard<std::mutex> lk(g->mu);
     unsigned long long c[CTL_WORDS];
-    CUDA_TRY(cudaMemcpy(c, g->ctl.p, sizeof c, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(c, g->tiers.ctl.p, sizeof c, cudaMemcpyDeviceToHost));
     for (int set = 0; set < 2; set++) {
         const unsigned long long *k = c + set * CTL_SET;
         out8[set * 4 + 0] = static_cast<int64_t>(k[1] + k[3]);          // S1 hand-offs (heavy + other)
@@ -954,11 +978,13 @@ extern "C" int abb_last_walk_tier_counts(abb_graph *g, int64_t *out8) {
 }
 
 extern "C" float abb_last_paths_ms(abb_graph *g) {
-    if (!g || !g->paths_timed) return -1.f;
+    if (!g) return -1.f;
     DeviceGuard dg(g->device);
+    std::lock_guard<std::mutex> lk(g->mu);   // both events of one call: another thread's call records them under the lock
+    if (!g->paths.timed) return -1.f;
     float ms = -1.f;
-    if (cudaEventSynchronize(g->ev[3]) != cudaSuccess) return -1.f;
-    if (cudaEventElapsedTime(&ms, g->ev[2], g->ev[3]) != cudaSuccess) return -1.f;
+    if (cudaEventSynchronize(g->paths.ev_end) != cudaSuccess) return -1.f;
+    if (cudaEventElapsedTime(&ms, g->paths.ev_start, g->paths.ev_end) != cudaSuccess) return -1.f;
     return ms;
 }
 
@@ -1036,117 +1062,118 @@ extern "C" int64_t abb_walk_result_d2h_bytes(const abb_walk_result *r) { return 
 // fails when a walk of either set (canonical, individual) outgrew the last storage tier; the walk's stream must be idle
 static int check_tier_fatal(abb_graph *g) {
     unsigned long long fatal = 0, fatal2 = 0;
-    CUDA_TRY(cudaMemcpy(&fatal, g->ctl.as<unsigned long long>() + CTL_FATAL, sizeof fatal, cudaMemcpyDeviceToHost));
-    CUDA_TRY(cudaMemcpy(&fatal2, g->ctl.as<unsigned long long>() + CTL_SET + CTL_FATAL, sizeof fatal2, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(&fatal, g->tiers.ctl.as<unsigned long long>() + CTL_FATAL, sizeof fatal, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(&fatal2, g->tiers.ctl.as<unsigned long long>() + CTL_SET + CTL_FATAL, sizeof fatal2, cudaMemcpyDeviceToHost));
     if (fatal || fatal2) return fail(ABB_ERR_CAPACITY, "a traversal outgrew the global scratch tier (more than n_nodes+4096 queue entries)");
     return ABB_OK;
 }
 
-// the non-zero histogram columns and the largest count of nq rows, into g->hist_info once st has been synchronised
+// the non-zero histogram columns and the largest count of nq rows, into g->staging.hist_info once st has been synchronised
 static int scan_hist_columns(abb_graph *g, const uint32_t *q_hist, int64_t nq, cudaStream_t st) {
-    if (int rc = g->d_histinfo.ensure(2 * sizeof(unsigned long long))) return rc;
-    CUDA_TRY(cudaMemsetAsync(g->d_histinfo.p, 0, 2 * sizeof(unsigned long long), st));
+    if (int rc = g->staging.hist_info_dev.ensure(2 * sizeof(unsigned long long))) return rc;
+    CUDA_TRY(cudaMemsetAsync(g->staging.hist_info_dev.p, 0, 2 * sizeof(unsigned long long), st));
     if (int rc = LAUNCH(hist_columns_kernel, static_cast<unsigned>(g->sm_count) * 8, 256, 0, st, q_hist, nq * ABB_N_ENTITY_TYPES,
-                        g->d_histinfo.as<unsigned long long>()))
+                        g->staging.hist_info_dev.as<unsigned long long>()))
         return rc;
-    CUDA_TRY(cudaMemcpyAsync(g->hist_info, g->d_histinfo.p, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(g->staging.hist_info, g->staging.hist_info_dev.p, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
     return ABB_OK;
 }
 
-// r's packed-histogram layout from g->hist_info: the non-zero columns, at 2 bytes per count when every count fits
+// r's packed-histogram layout from g->staging.hist_info: the non-zero columns, at 2 bytes per count when every count fits
 static HistCols hist_layout(const abb_graph *g, abb_walk_result *r) {
     HistCols hc{};
     r->hist_is_packed = true;
-    r->hist_mask = static_cast<uint32_t>(g->hist_info[0]);
+    r->hist_mask = static_cast<uint32_t>(g->staging.hist_info[0]);
     for (int t = 0; t < ABB_N_ENTITY_TYPES; t++) if (r->hist_mask >> t & 1u) hc.col[hc.k++] = static_cast<uint8_t>(t);
     r->hist_k = hc.k;
-    r->hist_width = g->hist_info[1] < 65536ull ? 2 : 4;
+    r->hist_width = g->staging.hist_info[1] < 65536ull ? 2 : 4;
     return hc;
 }
 
 // size hints for the next host walk: the largest node arena so far and the last batch; for a plain walk (one root per query, no
 // parents / depths / edges / targets) also what the chunked path sizes its pieces from
 static void note_walk_size(abb_graph *g, const abb_walk_spec *spec, int64_t nq, int64_t nodes, bool plain) {
-    g->hint_nodes = std::max(g->hint_nodes, nodes);
-    g->hint_nq = nq; g->hint_last_nodes = nodes;
+    g->staging.hint_nodes = std::max(g->staging.hint_nodes, nodes);
+    g->staging.hint_nq = nq; g->staging.hint_last_nodes = nodes;
     if (!plain) return;
-    if (g->plain_nq != nq || memcmp(&g->plain_spec, spec, sizeof *spec) != 0) g->chunk_hint_nq = -1;
-    g->plain_spec = *spec; g->plain_nq = nq; g->plain_nodes = nodes;
+    if (g->staging.plain_nq != nq || memcmp(&g->staging.plain_spec, spec, sizeof *spec) != 0) g->chunked.hint_nq = -1;
+    g->staging.plain_spec = *spec; g->staging.plain_nq = nq; g->staging.plain_nodes = nodes;
 }
 
 // stage inputs, run (re-run once if the arenas were too small), leave results on the device
 // `direct_nodes`: when the result size is known from the previous call, the walk kernels write the node arena
 // straight into that pinned host block (UVA), so the PCIe transfer of the largest output overlaps the traversal
 // instead of following it; if the estimate turns out too small the walk is re-run into a device arena.
-// `roots_staged`: the caller has already copied the single roots into g->d_roots on g->stream (sized for nq + 1).
+// `roots_staged`: the caller has already copied the single roots into g->staging.roots on g->stream (sized for nq + 1).
 static int walk_device_stage(abb_graph *g, const abb_walk_spec *spec, const int32_t *roots, const int64_t *root_off, const int32_t *targets,
                              int64_t nq, abb_walk_io *io_out, unsigned long long (&totals)[3], int64_t *h2d, HostBlock *direct_nodes = nullptr,
                              bool roots_staged = false) {
     cudaStream_t st = g->stream;
+    WalkStaging &S = g->staging;
     const uint32_t fl = spec->flags;
-    g->hist_info_valid = false;
+    S.hist_info_valid = false;
     const int64_t n_roots = root_off ? root_off[nq] : nq;
     if (n_roots < 0) return fail(ABB_ERR_ARG, "bad root_off");
     const size_t q1 = static_cast<size_t>(nq) + 1;
     int rc = ABB_OK;
-    ENS(d_roots, (n_roots + 1) * 4);
-    if (root_off) ENS(d_root_off, q1 * 8);
-    if (fl & ABB_WALK_TARGET) ENS(d_targets, q1 * 4);
-    ENS(d_qstart, q1 * 8); ENS(d_qcount, q1 * 4); ENS(d_qmaxd, q1 * 4); ENS(d_qflags, q1 * 4);
-    if (fl & ABB_WALK_EDGES) { ENS(d_qestart, q1 * 8); ENS(d_qecount, q1 * 8); }
-    if (fl & ABB_WALK_HIST) ENS(d_qhist, q1 * ABB_N_ENTITY_TYPES * 4);
-    ENS(d_totals, 3 * sizeof(unsigned long long));
+    ENS(S.roots, (n_roots + 1) * 4);
+    if (root_off) ENS(S.root_off, q1 * 8);
+    if (fl & ABB_WALK_TARGET) ENS(S.targets, q1 * 4);
+    ENS(S.qstart, q1 * 8); ENS(S.qcount, q1 * 4); ENS(S.qmaxd, q1 * 4); ENS(S.qflags, q1 * 4);
+    if (fl & ABB_WALK_EDGES) { ENS(S.qestart, q1 * 8); ENS(S.qecount, q1 * 8); }
+    if (fl & ABB_WALK_HIST) ENS(S.qhist, q1 * ABB_N_ENTITY_TYPES * 4);
+    ENS(S.totals, 3 * sizeof(unsigned long long));
     if (rc) return rc;
     *h2d = 0;
-    if (n_roots && !roots_staged) { CUDA_TRY(cudaMemcpyAsync(g->d_roots.p, roots, static_cast<size_t>(n_roots) * 4, cudaMemcpyHostToDevice, st)); *h2d += n_roots * 4; }
-    if (root_off) { CUDA_TRY(cudaMemcpyAsync(g->d_root_off.p, root_off, q1 * 8, cudaMemcpyHostToDevice, st)); *h2d += static_cast<int64_t>(q1) * 8; }
-    if (fl & ABB_WALK_TARGET) { CUDA_TRY(cudaMemcpyAsync(g->d_targets.p, targets, static_cast<size_t>(nq) * 4, cudaMemcpyHostToDevice, st)); *h2d += nq * 4; }
+    if (n_roots && !roots_staged) { CUDA_TRY(cudaMemcpyAsync(S.roots.p, roots, static_cast<size_t>(n_roots) * 4, cudaMemcpyHostToDevice, st)); *h2d += n_roots * 4; }
+    if (root_off) { CUDA_TRY(cudaMemcpyAsync(S.root_off.p, root_off, q1 * 8, cudaMemcpyHostToDevice, st)); *h2d += static_cast<int64_t>(q1) * 8; }
+    if (fl & ABB_WALK_TARGET) { CUDA_TRY(cudaMemcpyAsync(S.targets.p, targets, static_cast<size_t>(nq) * 4, cudaMemcpyHostToDevice, st)); *h2d += nq * 4; }
 
-    int64_t node_cap = std::max<int64_t>({g->hint_nodes, nq * 8, 1 << 16});
-    int64_t edge_cap = (fl & ABB_WALK_EDGES) ? std::max<int64_t>({g->hint_edges, nq * 16, 1 << 16}) : 0;
-    bool direct = direct_nodes && g->zero_copy && g->hint_nodes > 0 && !(fl & (ABB_WALK_PARENTS | ABB_WALK_DEPTHS | ABB_WALK_EDGES));
+    int64_t node_cap = std::max<int64_t>({S.hint_nodes, nq * 8, 1 << 16});
+    int64_t edge_cap = (fl & ABB_WALK_EDGES) ? std::max<int64_t>({S.hint_edges, nq * 16, 1 << 16}) : 0;
+    bool direct = direct_nodes && S.zero_copy && S.hint_nodes > 0 && !(fl & (ABB_WALK_PARENTS | ABB_WALK_DEPTHS | ABB_WALK_EDGES));
     if (direct) {
         // same batch size as last time: its exact need plus a little; otherwise scale the last per-query average generously, but
         // to no more than twice the largest arena any call has needed (a small batch of heavy sources, scaled to millions of
         // sources, would ask for more than the device holds; an estimate that is too small only costs a re-run into a device arena)
-        node_cap = (nq == g->hint_nq) ? g->hint_last_nodes + g->hint_last_nodes / 64 + 4096 + (g->align_direct ? 32 * nq : 0)
-                                      : std::min(static_cast<int64_t>(1.5 * static_cast<double>(g->hint_last_nodes) / std::max<int64_t>(g->hint_nq, 1) * nq) + 4096,
+        node_cap = (nq == S.hint_nq) ? S.hint_last_nodes + S.hint_last_nodes / 64 + 4096 + (g->tiers.align_direct ? 32 * nq : 0)
+                                      : std::min(static_cast<int64_t>(1.5 * static_cast<double>(S.hint_last_nodes) / std::max<int64_t>(S.hint_nq, 1) * nq) + 4096,
                                                  2 * node_cap);
         direct = direct_nodes->alloc(static_cast<size_t>(node_cap) * 4);
     }
     for (int attempt = 0; attempt < 3; attempt++) {
-        if (!direct) ENS(d_nodes, node_cap * 4);
-        if (fl & ABB_WALK_PARENTS) ENS(d_parent, node_cap * 4);
-        if (fl & ABB_WALK_DEPTHS) ENS(d_depth, node_cap * 4);
-        if (fl & ABB_WALK_EDGES) ENS(d_edges, edge_cap * 4);
+        if (!direct) ENS(S.nodes, node_cap * 4);
+        if (fl & ABB_WALK_PARENTS) ENS(S.parent, node_cap * 4);
+        if (fl & ABB_WALK_DEPTHS) ENS(S.depth, node_cap * 4);
+        if (fl & ABB_WALK_EDGES) ENS(S.edges, edge_cap * 4);
         if (rc) return rc;
         abb_walk_io io{};
-        io.n_queries = nq; io.roots = g->d_roots.as<int32_t>(); io.root_off = root_off ? g->d_root_off.as<int64_t>() : nullptr;
-        io.targets = (fl & ABB_WALK_TARGET) ? g->d_targets.as<int32_t>() : nullptr;
-        io.q_start = g->d_qstart.as<int64_t>(); io.q_count = g->d_qcount.as<int32_t>(); io.q_maxd = g->d_qmaxd.as<int32_t>(); io.q_flags = g->d_qflags.as<int32_t>();
-        io.q_estart = g->d_qestart.as<int64_t>(); io.q_ecount = g->d_qecount.as<int64_t>(); io.q_hist = g->d_qhist.as<uint32_t>();
-        io.nodes = direct ? direct_nodes->as<int32_t>() : g->d_nodes.as<int32_t>();
-        io.parent = g->d_parent.as<int32_t>(); io.depth = g->d_depth.as<int32_t>(); io.node_cap = node_cap;
-        io.edges = g->d_edges.as<uint32_t>(); io.edge_cap = edge_cap; io.totals = g->d_totals.as<unsigned long long>();
-        CUDA_TRY(cudaEventRecord(g->ev[0], st));
-        g->slice_align = (direct && g->align_direct) ? 32 : 0;
-        CUDA_TRY(cudaMemsetAsync(g->d_totals.as<unsigned long long>() + 2, 0, sizeof(unsigned long long), st));
+        io.n_queries = nq; io.roots = S.roots.as<int32_t>(); io.root_off = root_off ? S.root_off.as<int64_t>() : nullptr;
+        io.targets = (fl & ABB_WALK_TARGET) ? S.targets.as<int32_t>() : nullptr;
+        io.q_start = S.qstart.as<int64_t>(); io.q_count = S.qcount.as<int32_t>(); io.q_maxd = S.qmaxd.as<int32_t>(); io.q_flags = S.qflags.as<int32_t>();
+        io.q_estart = S.qestart.as<int64_t>(); io.q_ecount = S.qecount.as<int64_t>(); io.q_hist = S.qhist.as<uint32_t>();
+        io.nodes = direct ? direct_nodes->as<int32_t>() : S.nodes.as<int32_t>();
+        io.parent = S.parent.as<int32_t>(); io.depth = S.depth.as<int32_t>(); io.node_cap = node_cap;
+        io.edges = S.edges.as<uint32_t>(); io.edge_cap = edge_cap; io.totals = S.totals.as<unsigned long long>();
+        CUDA_TRY(cudaEventRecord(S.ev_start, st));
+        g->tiers.slice_align = (direct && g->tiers.align_direct) ? 32 : 0;
+        CUDA_TRY(cudaMemsetAsync(S.totals.as<unsigned long long>() + 2, 0, sizeof(unsigned long long), st));
         int erc = enqueue_walk(g, spec, &io, st);
-        g->slice_align = 0;
+        g->tiers.slice_align = 0;
         if (erc) return erc;
-        CUDA_TRY(cudaEventRecord(g->ev[1], st));
-        g->walk_timed = true;
-        const bool scan_hist = (fl & ABB_WALK_HIST) && g->hist_pack && nq >= 1024;
+        CUDA_TRY(cudaEventRecord(S.ev_end, st));
+        S.timed = true;
+        const bool scan_hist = (fl & ABB_WALK_HIST) && S.hist_pack && nq >= 1024;
         if (scan_hist) if ((rc = scan_hist_columns(g, io.q_hist, nq, st))) return rc;
-        CUDA_TRY(cudaMemcpyAsync(totals, g->d_totals.p, 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(totals, S.totals.p, 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaStreamSynchronize(st));
-        g->hist_info_valid = scan_hist;
+        S.hist_info_valid = scan_hist;
         if ((rc = check_tier_fatal(g))) return rc;
         *io_out = io;
         const bool fits = static_cast<int64_t>(totals[0]) <= node_cap && (!(fl & ABB_WALK_EDGES) || static_cast<int64_t>(totals[1]) <= edge_cap);
         const bool plain = !root_off && !(fl & (ABB_WALK_PARENTS | ABB_WALK_DEPTHS | ABB_WALK_EDGES | ABB_WALK_TARGET));
         note_walk_size(g, spec, nq, static_cast<int64_t>(totals[0]), fits && plain);
-        g->hint_edges = std::max<int64_t>(g->hint_edges, static_cast<int64_t>(totals[1]));
+        S.hint_edges = std::max<int64_t>(S.hint_edges, static_cast<int64_t>(totals[1]));
         if (fits) return ABB_OK;
         if (direct) { direct_nodes->release(); direct = false; }     // estimate too small: fall back to a device arena
         node_cap = std::max<int64_t>(node_cap, static_cast<int64_t>(totals[0]));
@@ -1162,8 +1189,8 @@ static int walk_collect(abb_graph *g, const abb_walk_spec *spec, const abb_walk_
                         abb_walk_result **out, bool sync, HostBlock *direct_nodes = nullptr, bool with_slices = true) {
     cudaStream_t st = g->stream;
     if (!sync) {
-        CUDA_TRY(cudaEventRecord(g->ev_copy, g->stream));
-        CUDA_TRY(cudaStreamWaitEvent(g->copy_stream, g->ev_copy, 0));
+        CUDA_TRY(cudaEventRecord(g->staging.ev_copy, g->stream));
+        CUDA_TRY(cudaStreamWaitEvent(g->copy_stream, g->staging.ev_copy, 0));
         st = g->copy_stream;
     }
     const uint32_t fl = spec->flags;
@@ -1177,8 +1204,8 @@ static int walk_collect(abb_graph *g, const abb_walk_spec *spec, const abb_walk_
     bool ok = (!with_slices || r->q_start.alloc(q * 8)) && r->q_count.alloc(q * 4) && r->q_maxd.alloc(q * 4) && r->q_flags.alloc(q * 4) &&
               (have_nodes || !with_slices || r->nodes.alloc(tn * 4));
     if (fl & ABB_WALK_EDGES) ok = ok && r->q_estart.alloc(q * 8) && r->q_ecount.alloc(q * 8) && r->edges.alloc(te * 4);
-    const bool pack = (fl & ABB_WALK_HIST) && g->hist_info_valid;
-    g->hist_info_valid = false;
+    const bool pack = (fl & ABB_WALK_HIST) && g->staging.hist_info_valid;
+    g->staging.hist_info_valid = false;
     const HistCols hc = pack ? hist_layout(g, r.get()) : HistCols{};
     if (pack) ok = ok && (hc.k == 0 || r->q_hist_packed.alloc(q * hc.k * r->hist_width));
     else if (fl & ABB_WALK_HIST) ok = ok && r->q_hist.alloc(q * ABB_N_ENTITY_TYPES * 4);
@@ -1193,13 +1220,13 @@ static int walk_collect(abb_graph *g, const abb_walk_spec *spec, const abb_walk_
     if (pack) {
         if (hc.k) {
             const size_t pbytes = q * hc.k * r->hist_width;
-            if (int rc = g->d_hist_packed.ensure(pbytes)) return rc;
+            if (int rc = g->staging.hist_packed.ensure(pbytes)) return rc;
             const unsigned grid = static_cast<unsigned>(g->sm_count) * 8;
-            const int rc = r->hist_width == 2 ? LAUNCH(hist_pack_kernel<uint16_t>, grid, 256, 0, st, io.q_hist, nq, hc, g->d_hist_packed.as<uint16_t>())
-                                              : LAUNCH(hist_pack_kernel<uint32_t>, grid, 256, 0, st, io.q_hist, nq, hc, g->d_hist_packed.as<uint32_t>());
+            const int rc = r->hist_width == 2 ? LAUNCH(hist_pack_kernel<uint16_t>, grid, 256, 0, st, io.q_hist, nq, hc, g->staging.hist_packed.as<uint16_t>())
+                                              : LAUNCH(hist_pack_kernel<uint32_t>, grid, 256, 0, st, io.q_hist, nq, hc, g->staging.hist_packed.as<uint32_t>());
             if (rc) return rc;
             d2h.keep(cudaGetLastError());
-            d2h(r->q_hist_packed, g->d_hist_packed.p, pbytes);
+            d2h(r->q_hist_packed, g->staging.hist_packed.p, pbytes);
         }
     } else if (fl & ABB_WALK_HIST) d2h(r->q_hist, io.q_hist, q * ABB_N_ENTITY_TYPES * 4);
     if (fl & ABB_WALK_PARENTS) d2h(r->parent, io.parent, tn * 4);
@@ -1226,57 +1253,59 @@ __global__ void add_base_kernel(int64_t *q_start, int64_t n, int64_t base) {
 
 static bool chunked_applies(const abb_graph *g, const abb_walk_spec *spec, const int64_t *root_off, const int32_t *targets, int64_t nq) {
     const uint32_t fl = spec->flags;
-    return g->chunks > 1 && nq >= g->chunk_min && nq >= 2 * g->chunks && !root_off && !targets &&
-           !(fl & (ABB_WALK_PARENTS | ABB_WALK_DEPTHS | ABB_WALK_EDGES | ABB_WALK_TARGET)) && g->plain_nq == nq && g->plain_nodes > 0 &&
-           memcmp(&g->plain_spec, spec, sizeof *spec) == 0;
+    return g->chunked.chunks > 1 && nq >= g->chunked.chunk_min && nq >= 2 * g->chunked.chunks && !root_off && !targets &&
+           !(fl & (ABB_WALK_PARENTS | ABB_WALK_DEPTHS | ABB_WALK_EDGES | ABB_WALK_TARGET)) && g->staging.plain_nq == nq && g->staging.plain_nodes > 0 &&
+           memcmp(&g->staging.plain_spec, spec, sizeof *spec) == 0;
 }
 
 static int walk_host_chunked(abb_graph *g, const abb_walk_spec *spec, const int32_t *roots, int64_t nq, abb_walk_result **out) {
     NvtxRange nvtx_("walk_host_chunked");
     cudaStream_t st = g->stream, cst = g->copy_stream;
+    WalkStaging &S = g->staging;
+    ChunkedWalk &C = g->chunked;
     const uint32_t fl = spec->flags;
-    const int K = g->chunks;
+    const int K = C.chunks;
     const size_t q = static_cast<size_t>(nq), q1 = q + 1;
     const bool hist = (fl & ABB_WALK_HIST) != 0;
     int rc = ABB_OK;
-    ENS(d_roots, q1 * 4); ENS(d_qstart, q1 * 8); ENS(d_qcount, q1 * 4); ENS(d_qmaxd, q1 * 4); ENS(d_qflags, q1 * 4);
-    if (hist) ENS(d_qhist, q1 * ABB_N_ENTITY_TYPES * 4);
-    ENS(d_totals, 3 * sizeof(unsigned long long));
-    ENS(ck_roots, q1 * 4); ENS(ck_sig, q1 * 8); ENS(ck_key, q1 * 4); ENS(ck_key2, q1 * 4); ENS(ck_idx, q1 * 4); ENS(ck_order, q1 * 4); ENS(ck_counts, 64 * 8);
-    ENS(ck_qstart, q1 * 8); ENS(ck_qcount, q1 * 4); ENS(ck_qmaxd, q1 * 4); ENS(ck_qflags, q1 * 4);
+    ENS(S.roots, q1 * 4); ENS(S.qstart, q1 * 8); ENS(S.qcount, q1 * 4); ENS(S.qmaxd, q1 * 4); ENS(S.qflags, q1 * 4);
+    if (hist) ENS(S.qhist, q1 * ABB_N_ENTITY_TYPES * 4);
+    ENS(S.totals, 3 * sizeof(unsigned long long));
+    ENS(C.roots, q1 * 4); ENS(C.sig, q1 * 8); ENS(C.key, q1 * 4); ENS(C.key2, q1 * 4); ENS(C.idx, q1 * 4); ENS(C.order, q1 * 4); ENS(C.counts, 64 * 8);
+    ENS(C.qstart, q1 * 8); ENS(C.qcount, q1 * 4); ENS(C.qmaxd, q1 * 4); ENS(C.qflags, q1 * 4);
     if (rc) return rc;
-    const bool have_hint = g->chunk_hint_nq == nq && static_cast<int>(g->chunk_hint.size()) == K;
+    const bool have_hint = C.hint_nq == nq && static_cast<int>(C.hint.size()) == K;
     // host arena: last total plus slack (the one-piece zero-copy pass pads slices, so its total is an upper bound already)
-    const int64_t host_cap = g->plain_nodes + g->plain_nodes / (have_hint ? 64 : 8) + 4096ll * K;
+    const int64_t host_cap = S.plain_nodes + S.plain_nodes / (have_hint ? 64 : 8) + 4096ll * K;
     std::unique_ptr<abb_walk_result> r(new abb_walk_result());
     r->nq = nq; r->flags = fl;
     if (!(r->q_start.alloc(q * 8) && r->q_count.alloc(q * 4) && r->q_maxd.alloc(q * 4) && r->q_flags.alloc(q * 4) && r->nodes.alloc(static_cast<size_t>(host_cap) * 4)))
         return fail(ABB_ERR_NOMEM, "pinned host allocation failed");
     auto drain = [&]() { cudaStreamSynchronize(st); cudaStreamSynchronize(cst); };
     const unsigned qblocks = static_cast<unsigned>((nq + 255) / 256);
-    CUDA_TRY(cudaMemcpyAsync(g->d_roots.p, roots, q * 4, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(S.roots.p, roots, q * 4, cudaMemcpyHostToDevice, st));
     r->h2d = nq * 4;
-    CUDA_TRY(cudaEventRecord(g->ev[0], st));
+    CUDA_TRY(cudaEventRecord(S.ev_start, st));
     // partition: chunk = frontier signature mod K when the walk de-duplicates (a frontier group is never split), contiguous ranges otherwise
     abb_walk_io probe{}; probe.n_queries = nq;
     const bool by_sig = dedup_applies(g, spec, &probe);
     unsigned long long *sig = nullptr;
     if (by_sig) {
-        sig = g->ck_sig.as<unsigned long long>();
-        if ((rc = LAUNCH(dedup_sig_kernel, qblocks, 256, 0, st, g->v, *spec, g->d_roots.as<int32_t>(), nq, sig, nullptr))) { drain(); return rc; }
+        sig = C.sig.as<unsigned long long>();
+        if ((rc = LAUNCH(dedup_sig_kernel, qblocks, 256, 0, st, g->v, *spec, S.roots.as<int32_t>(), nq, sig, nullptr))) { drain(); return rc; }
     }
-    CUDA_TRY(cudaMemsetAsync(g->ck_counts.p, 0, 64 * 8, st));
-    if ((rc = LAUNCH(chunk_key_kernel, qblocks, 256, 0, st, sig, nq, K, g->ck_key.as<uint32_t>(), g->ck_idx.as<int32_t>(), g->ck_counts.as<unsigned long long>()))) {
+    CUDA_TRY(cudaMemsetAsync(C.counts.p, 0, 64 * 8, st));
+    if ((rc = LAUNCH(chunk_key_kernel, qblocks, 256, 0, st, sig, nq, K, C.key.as<uint32_t>(), C.idx.as<int32_t>(), C.counts.as<unsigned long long>()))) {
         drain(); return rc;
     }
-    if ((rc = cub_run(g->ck_tmp, [&](void *t, size_t &b) {
-             return cub::DeviceRadixSort::SortPairs(t, b, g->ck_key.as<uint32_t>(), g->ck_key2.as<uint32_t>(), g->ck_idx.as<int32_t>(), g->ck_order.as<int32_t>(),
+    if ((rc = cub_run(C.tmp, [&](void *t, size_t &b) {
+             return cub::DeviceRadixSort::SortPairs(t, b, C.key.as<uint32_t>(), C.key2.as<uint32_t>(), C.idx.as<int32_t>(), C.order.as<int32_t>(),
                                                     static_cast<int>(nq), 0, 6, st);
          }))) { drain(); return rc; }
-    const int32_t *order = g->ck_order.as<int32_t>();      // order[i] = caller index of the i-th query in chunk order
-    if ((rc = LAUNCH(gather_i32_kernel, qblocks, 256, 0, st, g->d_roots.as<int32_t>(), order, g->ck_roots.as<int32_t>(), nq))) { drain(); return rc; }
+    const int32_t *order = C.order.as<int32_t>();      // order[i] = caller index of the i-th query in chunk order
+    if ((rc = LAUNCH(gather_i32_kernel, qblocks, 256, 0, st, S.roots.as<int32_t>(), order, C.roots.as<int32_t>(), nq))) { drain(); return rc; }
     unsigned long long counts[64] = {0};
-    CUDA_TRY(cudaMemcpyAsync(counts, g->ck_counts.p, 64 * 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(counts, C.counts.p, 64 * 8, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     std::vector<int64_t> produced(static_cast<size_t>(K), 0);
     int64_t node_base = 0, b0 = 0;
@@ -1285,25 +1314,25 @@ static int walk_host_chunked(abb_graph *g, const abb_walk_spec *spec, const int3
         const int64_t nk = static_cast<int64_t>(counts[k]);
         const int set = k & 1;
         if (!nk) continue;
-        DevBuf &arena = set ? g->d_nodes_alt : g->d_nodes;
-        int64_t cap = have_hint ? g->chunk_hint[static_cast<size_t>(k)] + g->chunk_hint[static_cast<size_t>(k)] / 64 + 4096
-                                : 2 * (g->plain_nodes / K) + 65536;
+        DevBuf &arena = set ? C.nodes_alt : S.nodes;
+        int64_t cap = have_hint ? C.hint[static_cast<size_t>(k)] + C.hint[static_cast<size_t>(k)] / 64 + 4096
+                                : 2 * (S.plain_nodes / K) + 65536;
         cap = std::max<int64_t>(cap, nk * 8);
         unsigned long long totals[3] = {0, 0, 0};
         bool done = false;
         for (int attempt = 0; attempt < 3 && !done; attempt++) {
-            if (static_cast<size_t>(cap) * 4 > arena.cap && copied[set]) CUDA_TRY(cudaEventSynchronize(g->ev_chunk_copied[set]));   // about to reallocate it
+            if (static_cast<size_t>(cap) * 4 > arena.cap && copied[set]) CUDA_TRY(cudaEventSynchronize(C.ev_copied[set]));   // about to reallocate it
             if ((rc = arena.ensure(static_cast<size_t>(cap) * 4))) { drain(); return rc; }
-            if (copied[set]) CUDA_TRY(cudaStreamWaitEvent(st, g->ev_chunk_copied[set], 0));       // the arena's previous contents have left
+            if (copied[set]) CUDA_TRY(cudaStreamWaitEvent(st, C.ev_copied[set], 0));       // the arena's previous contents have left
             abb_walk_io io{};
-            io.n_queries = nk; io.roots = g->ck_roots.as<int32_t>() + b0;
-            io.q_start = g->d_qstart.as<int64_t>() + b0; io.q_count = g->d_qcount.as<int32_t>() + b0; io.q_maxd = g->d_qmaxd.as<int32_t>() + b0;
-            io.q_flags = g->d_qflags.as<int32_t>() + b0;
-            io.q_hist = hist ? g->d_qhist.as<uint32_t>() + b0 * ABB_N_ENTITY_TYPES : nullptr;
-            io.nodes = arena.as<int32_t>(); io.node_cap = cap; io.totals = g->d_totals.as<unsigned long long>();
-            CUDA_TRY(cudaMemsetAsync(g->d_totals.as<unsigned long long>() + 2, 0, sizeof(unsigned long long), st));
+            io.n_queries = nk; io.roots = C.roots.as<int32_t>() + b0;
+            io.q_start = S.qstart.as<int64_t>() + b0; io.q_count = S.qcount.as<int32_t>() + b0; io.q_maxd = S.qmaxd.as<int32_t>() + b0;
+            io.q_flags = S.qflags.as<int32_t>() + b0;
+            io.q_hist = hist ? S.qhist.as<uint32_t>() + b0 * ABB_N_ENTITY_TYPES : nullptr;
+            io.nodes = arena.as<int32_t>(); io.node_cap = cap; io.totals = S.totals.as<unsigned long long>();
+            CUDA_TRY(cudaMemsetAsync(S.totals.as<unsigned long long>() + 2, 0, sizeof(unsigned long long), st));
             if (int erc = enqueue_walk(g, spec, &io, st)) { drain(); return erc; }
-            CUDA_TRY(cudaMemcpyAsync(totals, g->d_totals.p, 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(totals, S.totals.p, 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
             CUDA_TRY(cudaStreamSynchronize(st));
             if ((rc = check_tier_fatal(g))) { drain(); return rc; }
             if (static_cast<int64_t>(totals[0]) <= cap) done = true; else cap = static_cast<int64_t>(totals[0]) + 4096;
@@ -1313,68 +1342,68 @@ static int walk_host_chunked(abb_graph *g, const abb_walk_spec *spec, const int3
         produced[static_cast<size_t>(k)] = tot;
         if (node_base + tot > host_cap) {          // the host arena guess was too small: let the one-piece path redo the batch
             drain();
-            g->chunk_hint_nq = -1;
+            C.hint_nq = -1;
             return ABB_RETRY_UNCHUNKED;
         }
         if (node_base)
-            if ((rc = LAUNCH(add_base_kernel, static_cast<unsigned>((nk + 255) / 256), 256, 0, st, g->d_qstart.as<int64_t>() + b0, nk, node_base))) { drain(); return rc; }
-        CUDA_TRY(cudaEventRecord(g->ev_chunk_walked, st));
-        CUDA_TRY(cudaStreamWaitEvent(cst, g->ev_chunk_walked, 0));
+            if ((rc = LAUNCH(add_base_kernel, static_cast<unsigned>((nk + 255) / 256), 256, 0, st, S.qstart.as<int64_t>() + b0, nk, node_base))) { drain(); return rc; }
+        CUDA_TRY(cudaEventRecord(C.ev_walked, st));
+        CUDA_TRY(cudaStreamWaitEvent(cst, C.ev_walked, 0));
         if (tot) CUDA_TRY(cudaMemcpyAsync(r->nodes.as<int32_t>() + node_base, arena.p, static_cast<size_t>(tot) * 4, cudaMemcpyDeviceToHost, cst));
-        CUDA_TRY(cudaEventRecord(g->ev_chunk_copied[set], cst));
+        CUDA_TRY(cudaEventRecord(C.ev_copied[set], cst));
         copied[set] = true;
         node_base += tot;
         b0 += nk;
     }
     if (b0 != nq) { drain(); return fail(ABB_ERR_CUDA, "chunk partition lost queries (%lld of %lld)", static_cast<long long>(b0), static_cast<long long>(nq)); }
-    CUDA_TRY(cudaEventRecord(g->ev[1], st));
-    g->walk_timed = true;
+    CUDA_TRY(cudaEventRecord(S.ev_end, st));
+    S.timed = true;
     r->total_nodes = node_base;
     r->d2h += node_base * 4;
     // per-query results back into caller order, then to the host (the node copies of the last chunks are still in flight on the copy stream)
     const unsigned sgrid = static_cast<unsigned>(g->sm_count) * 8;
-    if ((rc = LAUNCH(scatter_rows_kernel<int64_t>, sgrid, 256, 0, st, g->d_qstart.as<int64_t>(), order, g->ck_qstart.as<int64_t>(), nq, 1)) ||
-        (rc = LAUNCH(scatter_rows_kernel<int32_t>, sgrid, 256, 0, st, g->d_qcount.as<int32_t>(), order, g->ck_qcount.as<int32_t>(), nq, 1)) ||
-        (rc = LAUNCH(scatter_rows_kernel<int32_t>, sgrid, 256, 0, st, g->d_qmaxd.as<int32_t>(), order, g->ck_qmaxd.as<int32_t>(), nq, 1)) ||
-        (rc = LAUNCH(scatter_rows_kernel<int32_t>, sgrid, 256, 0, st, g->d_qflags.as<int32_t>(), order, g->ck_qflags.as<int32_t>(), nq, 1))) {
+    if ((rc = LAUNCH(scatter_rows_kernel<int64_t>, sgrid, 256, 0, st, S.qstart.as<int64_t>(), order, C.qstart.as<int64_t>(), nq, 1)) ||
+        (rc = LAUNCH(scatter_rows_kernel<int32_t>, sgrid, 256, 0, st, S.qcount.as<int32_t>(), order, C.qcount.as<int32_t>(), nq, 1)) ||
+        (rc = LAUNCH(scatter_rows_kernel<int32_t>, sgrid, 256, 0, st, S.qmaxd.as<int32_t>(), order, C.qmaxd.as<int32_t>(), nq, 1)) ||
+        (rc = LAUNCH(scatter_rows_kernel<int32_t>, sgrid, 256, 0, st, S.qflags.as<int32_t>(), order, C.qflags.as<int32_t>(), nq, 1))) {
         drain(); return rc;
     }
-    const bool scan_hist = hist && g->hist_pack && nq >= 1024;
+    const bool scan_hist = hist && S.hist_pack && nq >= 1024;
     if (scan_hist) {
-        if ((rc = scan_hist_columns(g, g->d_qhist.as<uint32_t>(), nq, st))) { drain(); return rc; }
+        if ((rc = scan_hist_columns(g, S.qhist.as<uint32_t>(), nq, st))) { drain(); return rc; }
         CUDA_TRY(cudaStreamSynchronize(st));
     }
     Readback d2h{st, &r->d2h, cudaGetLastError()};
-    d2h(r->q_start, g->ck_qstart.p, q * 8); d2h(r->q_count, g->ck_qcount.p, q * 4); d2h(r->q_maxd, g->ck_qmaxd.p, q * 4); d2h(r->q_flags, g->ck_qflags.p, q * 4);
+    d2h(r->q_start, C.qstart.p, q * 8); d2h(r->q_count, C.qcount.p, q * 4); d2h(r->q_maxd, C.qmaxd.p, q * 4); d2h(r->q_flags, C.qflags.p, q * 4);
     if (scan_hist) {
         const HistCols hc = hist_layout(g, r.get());
         if (hc.k) {
             const size_t pbytes = q * hc.k * r->hist_width;
             if (!r->q_hist_packed.alloc(pbytes)) { drain(); return fail(ABB_ERR_NOMEM, "pinned host allocation failed"); }
-            if ((rc = g->d_hist_packed.ensure(pbytes))) { drain(); return rc; }
+            if ((rc = S.hist_packed.ensure(pbytes))) { drain(); return rc; }
             rc = r->hist_width == 2
-                     ? LAUNCH(hist_pack_scatter_kernel<uint16_t>, sgrid, 256, 0, st, g->d_qhist.as<uint32_t>(), order, nq, hc, g->d_hist_packed.as<uint16_t>())
-                     : LAUNCH(hist_pack_scatter_kernel<uint32_t>, sgrid, 256, 0, st, g->d_qhist.as<uint32_t>(), order, nq, hc, g->d_hist_packed.as<uint32_t>());
+                     ? LAUNCH(hist_pack_scatter_kernel<uint16_t>, sgrid, 256, 0, st, S.qhist.as<uint32_t>(), order, nq, hc, S.hist_packed.as<uint16_t>())
+                     : LAUNCH(hist_pack_scatter_kernel<uint32_t>, sgrid, 256, 0, st, S.qhist.as<uint32_t>(), order, nq, hc, S.hist_packed.as<uint32_t>());
             if (rc) { drain(); return rc; }
-            d2h(r->q_hist_packed, g->d_hist_packed.p, pbytes);
+            d2h(r->q_hist_packed, S.hist_packed.p, pbytes);
         }
     } else if (hist) {
         if (!r->q_hist.alloc(q * ABB_N_ENTITY_TYPES * 4)) { drain(); return fail(ABB_ERR_NOMEM, "pinned host allocation failed"); }
-        if ((rc = g->ck_qhist.ensure(q1 * ABB_N_ENTITY_TYPES * 4))) { drain(); return rc; }
-        if ((rc = LAUNCH(scatter_rows_kernel<uint32_t>, sgrid, 256, 0, st, g->d_qhist.as<uint32_t>(), order, g->ck_qhist.as<uint32_t>(), nq, ABB_N_ENTITY_TYPES))) {
+        if ((rc = C.qhist.ensure(q1 * ABB_N_ENTITY_TYPES * 4))) { drain(); return rc; }
+        if ((rc = LAUNCH(scatter_rows_kernel<uint32_t>, sgrid, 256, 0, st, S.qhist.as<uint32_t>(), order, C.qhist.as<uint32_t>(), nq, ABB_N_ENTITY_TYPES))) {
             drain(); return rc;
         }
-        d2h(r->q_hist, g->ck_qhist.p, q * ABB_N_ENTITY_TYPES * 4);
+        d2h(r->q_hist, C.qhist.p, q * ABB_N_ENTITY_TYPES * 4);
     }
     cudaError_t &e = d2h.err;
     if (e == cudaSuccess) e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(cst);
     if (e != cudaSuccess) { drain(); return fail(ABB_ERR_CUDA, "chunked walk failed: %s", cudaGetErrorString(e)); }
-    g->hist_info_valid = false;
+    S.hist_info_valid = false;
     note_walk_size(g, spec, nq, node_base, true);
-    g->chunk_hint = produced; g->chunk_hint_nq = nq;
-    g->last_host_chunks = K;
+    C.hint = produced; C.hint_nq = nq;
+    C.last_host_chunks = K;
     *out = r.release();
     return ABB_OK;
 }
@@ -1390,7 +1419,7 @@ extern "C" int abb_walk_host(abb_graph *g, const abb_walk_spec *spec, const int3
         const int crc = walk_host_chunked(g, spec, roots, n_queries, out);
         if (crc != ABB_RETRY_UNCHUNKED) return crc;
     }
-    g->last_host_chunks = 1;
+    g->chunked.last_host_chunks = 1;
     abb_walk_io io{}; unsigned long long totals[3] = {0, 0, 0}; int64_t h2d = 0;
     HostBlock direct;
     if (int rc = walk_device_stage(g, spec, roots, root_off, targets, n_queries, &io, totals, &h2d, &direct)) return rc;
@@ -1398,33 +1427,6 @@ extern "C" int abb_walk_host(abb_graph *g, const abb_walk_spec *spec, const int3
 }
 
 // ------------------------------------------------------------------ exposure-path rows
-static int ensure_server_table(abb_graph *g, cudaStream_t st) {
-    if (g->srv_table_ready) return ABB_OK;
-    const size_t n = static_cast<size_t>(g->v.n) + 1;
-    if (int rc = g->srv_cred.ensure(n * 4)) return rc;
-    if (int rc = g->srv_tool.ensure(n * 4)) return rc;
-    const unsigned grid = grid_for(g->v.n, 256, g->sm_count, 16);
-    if (int rc = LAUNCH(server_table_kernel, grid, 256, 0, st, g->v, g->srv_cred.as<int32_t>(), g->srv_tool.as<int32_t>())) return rc;
-    // principal rows of every server (paths.cuh server_rows_kernel): count, scan in place, fill
-    if (int rc = g->srv_roff.ensure(n * 8)) return rc;
-    int64_t *roff = g->srv_roff.as<int64_t>();
-    CUDA_TRY(cudaMemsetAsync(roff, 0, n * 8, st));
-    if (int rc = LAUNCH(server_rows_kernel<false>, grid, 256, 0, st, g->v, g->srv_cred.as<int32_t>(), g->srv_tool.as<int32_t>(), roff, nullptr, nullptr))
-        return rc;
-    if (int rc = scan_i64(g->p_scan_tmp, roff, roff, static_cast<int64_t>(n), st)) return rc;
-    int64_t total = 0;
-    CUDA_TRY(cudaMemcpyAsync(&total, roff + g->v.n, 8, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    if (int rc = g->srv_row.ensure(static_cast<size_t>(total + 1) * 16)) return rc;
-    if (int rc = g->srv_rel.ensure(static_cast<size_t>(total) + 16)) return rc;
-    if (int rc = LAUNCH(server_rows_kernel<true>, grid, 256, 0, st, g->v, g->srv_cred.as<int32_t>(), g->srv_tool.as<int32_t>(), roff, g->srv_row.as<int4>(),
-                        g->srv_rel.as<int8_t>()))
-        return rc;
-    CUDA_TRY(cudaStreamSynchronize(st));   // one-time: later launches may come on other streams
-    g->srv_table_ready = true;
-    return ABB_OK;
-}
-
 static unsigned warp_grid(const abb_graph *g, int64_t warps) {
     return static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>((warps + 7) / 8, static_cast<int64_t>(g->sm_count) * 8)));
 }
@@ -1442,94 +1444,115 @@ static unsigned row_grid(const abb_graph *g, K kernel, int &cached) {
     return static_cast<unsigned>(cached);
 }
 
-// the graph's parts of the exposure-path arguments: server table and exposure tables
-static PathsArgs paths_base(abb_graph *g) {
+// the graph's parts of the exposure-path arguments: server tables and exposure tables
+static PathsArgs paths_base(const GraphView &v, const ExposureTables &X) {
     PathsArgs A{};
-    A.g = g->v; A.srv_cred = g->srv_cred.as<int32_t>(); A.srv_tool = g->srv_tool.as<int32_t>();
-    A.srv_roff = g->srv_roff.as<int64_t>(); A.srv_row = g->srv_row.as<int4>(); A.srv_rel = g->srv_rel.as<int8_t>();
-    A.x_vs = g->x_vs.as<uint8_t>(); A.x_loff = g->x_loff.as<int64_t>(); A.x_link = g->x_link.as<LinkRec>(); A.x_rows = g->x_rows.as<int32_t>();
-    A.x_toff = g->x_toff.as<int64_t>(); A.t_row = g->x_trow.as<int4>(); A.t_rel = g->x_trel.as<int8_t>(); A.x_overflow = g->x_overflow.as<unsigned>();
+    A.g = v; A.srv_cred = X.srv_cred.as<int32_t>(); A.srv_tool = X.srv_tool.as<int32_t>();
+    A.srv_roff = X.srv_roff.as<int64_t>(); A.srv_row = X.srv_row.as<int4>(); A.srv_rel = X.srv_rel.as<int8_t>();
+    A.x_vs = X.vs.as<uint8_t>(); A.x_loff = X.loff.as<int64_t>(); A.x_link = X.link.as<LinkRec>(); A.x_rows = X.rows.as<int32_t>();
+    A.x_toff = X.toff.as<int64_t>(); A.t_row = X.trow.as<int4>(); A.t_rel = X.trel.as<int8_t>(); A.x_overflow = X.overflow.as<unsigned>();
     return A;
 }
 
-// Graph-constant exposure tables (paths.cuh): the links of every finding node, the template of every vulnerable source and the
-// rows of every finding node, built once per graph (count -> scan in place -> fill) and freed with it.  Synchronises the stream
-// to size the link and template arrays, and once more at the end: later calls may come on other streams.
+// Graph-constant exposure tables (paths.cuh), built once per graph and freed with it: the server tables (fan-out, and the principal
+// rows every server contributes to a template), then the links of every finding node, the template of every vulnerable source and
+// the rows of every finding node (count -> scan in place -> fill).  Built aside and installed only once complete: a failed build
+// leaves nothing behind.  Synchronises the stream to size the row, link and template arrays, and once more at the end: later calls
+// may come on other streams.
 static int ensure_exposure_tables(abb_graph *g, cudaStream_t st) {
-    if (g->x_tables_ready) return ABB_OK;
+    if (g->exposure) return ABB_OK;
     NvtxRange nvtx_("paths: graph-constant exposure tables");
-    if (int rc = ensure_server_table(g, st)) return rc;
+    std::unique_ptr<ExposureTables> X(new ExposureTables());
+    DevBuf &scan_tmp = g->paths.scan_tmp;
     const int64_t n = g->v.n;
     const size_t n1 = static_cast<size_t>(n) + 1;
-    int rc = ABB_OK;
-    if (!rc) rc = g->x_vs.alloc(n1);
-    if (!rc) rc = g->x_loff.alloc(n1 * 8);
-    if (!rc) rc = g->x_toff.alloc(n1 * 8);
-    if (!rc) rc = g->x_rows.alloc(n1 * 4);
-    if (!rc) rc = g->x_overflow.alloc(4);
+    if (int rc = X->srv_cred.ensure(n1 * 4)) return rc;
+    if (int rc = X->srv_tool.ensure(n1 * 4)) return rc;
+    const unsigned sgrid = grid_for(n, 256, g->sm_count, 16);
+    if (int rc = LAUNCH(server_table_kernel, sgrid, 256, 0, st, g->v, X->srv_cred.as<int32_t>(), X->srv_tool.as<int32_t>())) return rc;
+    // principal rows of every server (paths.cuh server_rows_kernel): count, scan in place, fill
+    if (int rc = X->srv_roff.ensure(n1 * 8)) return rc;
+    int64_t *roff = X->srv_roff.as<int64_t>();
+    CUDA_TRY(cudaMemsetAsync(roff, 0, n1 * 8, st));
+    if (int rc = LAUNCH(server_rows_kernel<false>, sgrid, 256, 0, st, g->v, X->srv_cred.as<int32_t>(), X->srv_tool.as<int32_t>(), roff, nullptr, nullptr))
+        return rc;
+    if (int rc = scan_i64(scan_tmp, roff, roff, static_cast<int64_t>(n1), st)) return rc;
+    int64_t total = 0;
+    CUDA_TRY(cudaMemcpyAsync(&total, roff + n, 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (int rc = X->srv_row.ensure(static_cast<size_t>(total + 1) * 16)) return rc;
+    if (int rc = X->srv_rel.ensure(static_cast<size_t>(total) + 16)) return rc;
+    if (int rc = LAUNCH(server_rows_kernel<true>, sgrid, 256, 0, st, g->v, X->srv_cred.as<int32_t>(), X->srv_tool.as<int32_t>(), roff, X->srv_row.as<int4>(),
+                        X->srv_rel.as<int8_t>()))
+        return rc;
+    int rc = X->vs.alloc(n1);
+    if (!rc) rc = X->loff.alloc(n1 * 8);
+    if (!rc) rc = X->toff.alloc(n1 * 8);
+    if (!rc) rc = X->rows.alloc(n1 * 4);
+    if (!rc) rc = X->overflow.alloc(4);
     if (rc) return rc;
-    PathsArgs A = paths_base(g);
+    PathsArgs A = paths_base(g->v, *X);
     CUDA_TRY(cudaMemsetAsync(A.x_vs, 0, n1, st));
     CUDA_TRY(cudaMemsetAsync(A.x_loff, 0, n1 * 8, st));
     CUDA_TRY(cudaMemsetAsync(A.x_toff, 0, n1 * 8, st));
     CUDA_TRY(cudaMemsetAsync(A.x_overflow, 0, 4, st));
     const unsigned grid = warp_grid(g, (n + 31) / 32);
     if ((rc = LAUNCH(node_links_kernel<false>, grid, 256, 0, st, A))) return rc;
-    if ((rc = scan_i64(g->p_scan_tmp, A.x_loff, A.x_loff, n + 1, st))) return rc;
+    if ((rc = scan_i64(scan_tmp, A.x_loff, A.x_loff, n + 1, st))) return rc;
     if ((rc = LAUNCH(template_kernel<false>, grid, 256, 0, st, A))) return rc;
-    if ((rc = scan_i64(g->p_scan_tmp, A.x_toff, A.x_toff, n + 1, st))) return rc;
+    if ((rc = scan_i64(scan_tmp, A.x_toff, A.x_toff, n + 1, st))) return rc;
     int64_t NL = 0, TR = 0;
     CUDA_TRY(cudaMemcpyAsync(&NL, A.x_loff + n, 8, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(&TR, A.x_toff + n, 8, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     // link records hold link and template offsets as int32
     if (NL >= (1ll << 31) - 1 || TR >= (1ll << 31) - 1) return fail(ABB_ERR_CAPACITY, "exposure tables: %lld links, %lld template rows (int32 offsets)", (long long)NL, (long long)TR);
-    if (!rc) rc = g->x_link.alloc(static_cast<size_t>(NL) * 16);
-    if (!rc) rc = g->x_trow.alloc(static_cast<size_t>(TR) * 16);
-    if (!rc) rc = g->x_trel.alloc(static_cast<size_t>(TR) * 2);
+    if (!rc) rc = X->link.alloc(static_cast<size_t>(NL) * 16);
+    if (!rc) rc = X->trow.alloc(static_cast<size_t>(TR) * 16);
+    if (!rc) rc = X->trel.alloc(static_cast<size_t>(TR) * 2);
     if (rc) return rc;
-    A = paths_base(g);
+    A = paths_base(g->v, *X);
     if ((rc = LAUNCH(template_kernel<true>, grid, 256, 0, st, A)) || (rc = LAUNCH(node_links_kernel<true>, grid, 256, 0, st, A))) return rc;
     unsigned overflow = 0;
     CUDA_TRY(cudaMemcpyAsync(&overflow, A.x_overflow, 4, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     if (overflow) return fail(ABB_ERR_CAPACITY, "exposure tables: a finding has 2^31 or more exposure-path rows");
-    g->x_tables_ready = true;
+    g->exposure = std::move(X);
     return ABB_OK;
 }
 
 // Count pass of the exposure-path pipeline (paths.cuh): each finding's row count and links gathered from the exposure tables, then
 // one exclusive scan into io.f_off.  Once the tables exist this neither synchronises nor, for a batch no larger than an earlier
-// one, allocates.  `link_counts` also writes each finding's link count (pl_lcnt) for the host result.
+// one, allocates.  `link_counts` also writes each finding's link count (f_lcnt) for the host result.
 static int enqueue_paths_count(abb_graph *g, const abb_paths_io *io, cudaStream_t st, bool link_counts = false) {
     NvtxRange nvtx_("paths: rows per finding");
     if (!io || io->n_findings < 0 || !io->f_off || (io->n_findings && !io->findings)) return fail(ABB_ERR_ARG, "bad paths io");
     if (io->n_findings >= (1ll << 31) - 2) return fail(ABB_ERR_ARG, "too many findings in one batch");
     if (int rc = ensure_exposure_tables(g, st)) return rc;
-    g->paths_args_valid = false;
+    g->paths.args_valid = false;
     const int64_t nf = io->n_findings;
-    int rc = g->pl_cnt.ensure(static_cast<size_t>(nf + 1) * 8);
-    if (!rc) rc = g->pl_link.ensure(static_cast<size_t>(nf + 1) * 8);
-    if (!rc && link_counts) rc = g->pl_lcnt.ensure(static_cast<size_t>(nf + 1) * 8);
+    int rc = g->paths.f_cnt.ensure(static_cast<size_t>(nf + 1) * 8);
+    if (!rc) rc = g->paths.f_link.ensure(static_cast<size_t>(nf + 1) * 8);
+    if (!rc && link_counts) rc = g->paths.f_lcnt.ensure(static_cast<size_t>(nf + 1) * 8);
     if (rc) return rc;
-    PathsArgs A = paths_base(g);
-    A.io = *io; A.f_cnt = g->pl_cnt.as<int64_t>(); A.f_link = g->pl_link.as<int2>(); A.f_lcnt = link_counts ? g->pl_lcnt.as<int64_t>() : nullptr;
+    PathsArgs A = paths_base(g->v, *g->exposure);
+    A.io = *io; A.f_cnt = g->paths.f_cnt.as<int64_t>(); A.f_link = g->paths.f_link.as<int2>(); A.f_lcnt = link_counts ? g->paths.f_lcnt.as<int64_t>() : nullptr;
     if ((rc = LAUNCH(finding_rows_kernel, static_cast<unsigned>((nf + 1 + 255) / 256), 256, 0, st, A))) return rc;
-    if ((rc = scan_i64(g->p_scan_tmp, A.f_cnt, io->f_off, nf + 1, st))) return rc;
-    g->paths_args = A;
-    g->paths_args_valid = true;
+    if ((rc = scan_i64(g->paths.scan_tmp, A.f_cnt, io->f_off, nf + 1, st))) return rc;
+    g->paths.args = A;
+    g->paths.args_valid = true;
     return ABB_OK;
 }
 
 static int enqueue_paths_fill(abb_graph *g, const abb_paths_io *io, cudaStream_t st) {
     if (!io || !io->f_off || !io->hops || !io->rels || !io->ncred || !io->ntool) return fail(ABB_ERR_ARG, "bad paths io");
     if (!io->n_findings) return ABB_OK;
-    if (!g->paths_args_valid || g->paths_args.io.findings != io->findings || g->paths_args.io.n_findings != io->n_findings || g->paths_args.io.f_off != io->f_off)
+    if (!g->paths.args_valid || g->paths.args.io.findings != io->findings || g->paths.args.io.n_findings != io->n_findings || g->paths.args.io.f_off != io->f_off)
         return fail(ABB_ERR_ARG, "abb_paths_fill_launch must follow abb_paths_count_launch for the same findings / f_off");
     if ((reinterpret_cast<uintptr_t>(io->hops) & 15) != 0 || (reinterpret_cast<uintptr_t>(io->rels) & 3) != 0) return fail(ABB_ERR_ARG, "io.hops must be 16-byte and io.rels 4-byte aligned");
-    PathsArgs A = g->paths_args;
+    PathsArgs A = g->paths.args;
     A.io = *io;
-    return LAUNCH(replicate_kernel, row_grid(g, replicate_kernel, g->replicate_grid), ROW_THREADS, 0, st, A);
+    return LAUNCH(replicate_kernel, row_grid(g, replicate_kernel, g->paths.replicate_grid), ROW_THREADS, 0, st, A);
 }
 
 extern "C" int abb_paths_count_launch(abb_graph *g, const abb_paths_io *io, void *stream) {
@@ -1538,7 +1561,7 @@ extern "C" int abb_paths_count_launch(abb_graph *g, const abb_paths_io *io, void
     DeviceGuard dg(g->device);
     std::lock_guard<std::mutex> lk(g->mu);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    CUDA_TRY(cudaEventRecord(g->ev[2], st));
+    CUDA_TRY(cudaEventRecord(g->paths.ev_start, st));
     return enqueue_paths_count(g, io, st);
 }
 extern "C" int abb_paths_fill_launch(abb_graph *g, const abb_paths_io *io, void *stream) {
@@ -1549,8 +1572,8 @@ extern "C" int abb_paths_fill_launch(abb_graph *g, const abb_paths_io *io, void 
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     int rc = enqueue_paths_fill(g, io, st);
     if (rc) return rc;
-    CUDA_TRY(cudaEventRecord(g->ev[3], st));
-    g->paths_timed = true;
+    CUDA_TRY(cudaEventRecord(g->paths.ev_end, st));
+    g->paths.timed = true;
     return ABB_OK;
 }
 
@@ -1627,58 +1650,59 @@ extern "C" int64_t abb_paths_result_d2h_bytes(const abb_paths_result *r) { retur
 // findings already on the device (d_findings) or staged from the host
 static int paths_run(abb_graph *g, const int32_t *h_findings, const int32_t *d_findings, int64_t nf, abb_paths_result **out, cudaStream_t st = nullptr) {
     if (!st) st = g->stream;
+    PathsWorkspace &P = g->paths;
     std::unique_ptr<abb_paths_result> r(new abb_paths_result());
     r->nf = nf;
     if (!r->findings.alloc(static_cast<size_t>(nf + 1) * 4)) return fail(ABB_ERR_NOMEM, "pinned host allocation failed");
     if (nf) memcpy(r->findings.p, h_findings, static_cast<size_t>(nf) * 4);
     if (!d_findings) {
-        if (int rc = g->p_findings.ensure(static_cast<size_t>(nf + 1) * 4)) return rc;
-        if (nf) { CUDA_TRY(cudaMemcpyAsync(g->p_findings.p, h_findings, static_cast<size_t>(nf) * 4, cudaMemcpyHostToDevice, st)); r->h2d += nf * 4; }
-        d_findings = g->p_findings.as<int32_t>();
+        if (int rc = P.findings.ensure(static_cast<size_t>(nf + 1) * 4)) return rc;
+        if (nf) { CUDA_TRY(cudaMemcpyAsync(P.findings.p, h_findings, static_cast<size_t>(nf) * 4, cudaMemcpyHostToDevice, st)); r->h2d += nf * 4; }
+        d_findings = P.findings.as<int32_t>();
     }
-    if (int rc = g->p_off.ensure(static_cast<size_t>(nf + 1) * 8)) return rc;
+    if (int rc = P.f_off.ensure(static_cast<size_t>(nf + 1) * 8)) return rc;
     abb_paths_io io{};
-    io.n_findings = nf; io.findings = d_findings; io.f_off = g->p_off.as<int64_t>();
-    CUDA_TRY(cudaEventRecord(g->ev[2], st));
+    io.n_findings = nf; io.findings = d_findings; io.f_off = P.f_off.as<int64_t>();
+    CUDA_TRY(cudaEventRecord(P.ev_start, st));
     if (int rc = enqueue_paths_count(g, &io, st, true)) return rc;
     // the batch's share of the exposure tables: its links (link counts scanned into link_off) and the templates of its distinct
     // vulnerable sources, in node order
-    const PathsArgs A = g->paths_args;
+    const PathsArgs A = P.args;
     const int64_t n = g->v.n;
-    int rc = g->pl_off.ensure(static_cast<size_t>(nf + 1) * 8);
+    int rc = P.link_off.ensure(static_cast<size_t>(nf + 1) * 8);
     if (rc) return rc;
-    int64_t *link_off = g->pl_off.as<int64_t>();
-    if ((rc = scan_i64(g->p_scan_tmp, A.f_lcnt, link_off, nf + 1, st))) return rc;
+    int64_t *link_off = P.link_off.as<int64_t>();
+    if ((rc = scan_i64(P.scan_tmp, A.f_lcnt, link_off, nf + 1, st))) return rc;
     int64_t NL = 0;
     CUDA_TRY(cudaMemcpyAsync(&NL, link_off + nf, 8, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     const int64_t nu_max = std::min<int64_t>(NL, n);
-    ENS(pl_vs, (NL + 2) * 4); ENS(pl_rel, NL + 16); ENS(pl_roff, (NL + 2) * 8); ENS(pl_toff, (NL + 2) * 8); ENS(pl_need, n + 16); ENS(pl_ulist, (n + 2) * 4);
-    ENS(pl_nu, 16); ENS(pt_cnt, (nu_max + 2) * 8); ENS(pt_off, (nu_max + 2) * 8); ENS(pt_off_node, (n + 2) * 8);
+    ENS(P.link_vs, (NL + 2) * 4); ENS(P.link_rel, NL + 16); ENS(P.link_roff, (NL + 2) * 8); ENS(P.link_toff, (NL + 2) * 8); ENS(P.need, n + 16); ENS(P.ulist, (n + 2) * 4);
+    ENS(P.nu, 16); ENS(P.t_cnt, (nu_max + 2) * 8); ENS(P.t_off, (nu_max + 2) * 8); ENS(P.t_off_node, (n + 2) * 8);
     if (rc) return rc;
-    int32_t *link_vs = g->pl_vs.as<int32_t>(), *ulist = g->pl_ulist.as<int32_t>();
-    int8_t *link_rel = g->pl_rel.as<int8_t>();
-    int64_t *link_roff = g->pl_roff.as<int64_t>(), *link_toff = g->pl_toff.as<int64_t>(), *t_cnt = g->pt_cnt.as<int64_t>(), *t_off = g->pt_off.as<int64_t>();
-    uint8_t *need = g->pl_need.as<uint8_t>();
-    unsigned long long *nu = g->pl_nu.as<unsigned long long>();
+    int32_t *link_vs = P.link_vs.as<int32_t>(), *ulist = P.ulist.as<int32_t>();
+    int8_t *link_rel = P.link_rel.as<int8_t>();
+    int64_t *link_roff = P.link_roff.as<int64_t>(), *link_toff = P.link_toff.as<int64_t>(), *t_cnt = P.t_cnt.as<int64_t>(), *t_off = P.t_off.as<int64_t>();
+    uint8_t *need = P.need.as<uint8_t>();
+    unsigned long long *nu = P.nu.as<unsigned long long>();
     CUDA_TRY(cudaMemsetAsync(need, 0, static_cast<size_t>(n) + 16, st));
     if ((rc = LAUNCH(batch_links_kernel, static_cast<unsigned>((nf + 1 + 255) / 256), 256, 0, st, A, link_off, link_vs, link_rel, link_roff, need))) return rc;
-    if ((rc = select_flagged(g->p_scan_tmp, need, ulist, nu, static_cast<int>(n), st))) return rc;
+    if ((rc = select_flagged(P.scan_tmp, need, ulist, nu, static_cast<int>(n), st))) return rc;
     CUDA_TRY(cudaMemsetAsync(t_cnt, 0, static_cast<size_t>(nu_max + 2) * 8, st));
     if (nu_max) if ((rc = LAUNCH(batch_template_counts_kernel, static_cast<unsigned>((nu_max + 255) / 256), 256, 0, st, A, ulist, nu, t_cnt))) return rc;
-    if ((rc = scan_i64(g->p_scan_tmp, t_cnt, t_off, nu_max + 1, st))) return rc;
+    if ((rc = scan_i64(P.scan_tmp, t_cnt, t_off, nu_max + 1, st))) return rc;
     int64_t TR = 0;
     CUDA_TRY(cudaMemcpyAsync(&TR, t_off + nu_max, 8, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
-    ENS(pt_row, (TR + 2) * 16); ENS(pt_rel, (TR + 2) * 2);
+    ENS(P.t_row, (TR + 2) * 16); ENS(P.t_rel, (TR + 2) * 2);
     if (rc) return rc;
-    int64_t *t_off_node = g->pt_off_node.as<int64_t>();
+    int64_t *t_off_node = P.t_off_node.as<int64_t>();
     if (nu_max)
-        if ((rc = LAUNCH(batch_templates_kernel, warp_grid(g, nu_max), 256, 0, st, A, ulist, nu, t_off, t_off_node, g->pt_row.as<int4>(), g->pt_rel.as<int8_t>())))
+        if ((rc = LAUNCH(batch_templates_kernel, warp_grid(g, nu_max), 256, 0, st, A, ulist, nu, t_off, t_off_node, P.t_row.as<int4>(), P.t_rel.as<int8_t>())))
             return rc;
     if (NL) if ((rc = LAUNCH(batch_link_toff_kernel, static_cast<unsigned>((NL + 255) / 256), 256, 0, st, NL, link_vs, t_off_node, link_toff))) return rc;
-    CUDA_TRY(cudaEventRecord(g->ev[3], st));
-    g->paths_timed = true;
+    CUDA_TRY(cudaEventRecord(P.ev_end, st));
+    P.timed = true;
     const size_t n1 = static_cast<size_t>(nf) + 1;
     r->n_links = NL; r->n_trows = TR;
     bool ok = r->off.alloc(n1 * 8) && r->link_off.alloc(n1 * 8) && r->link_vs.alloc(NL * 4) && r->link_rel.alloc(NL) && r->link_roff.alloc((NL + 1) * 8) &&
@@ -1686,7 +1710,7 @@ static int paths_run(abb_graph *g, const int32_t *h_findings, const int32_t *d_f
     if (!ok) return fail(ABB_ERR_NOMEM, "pinned host allocation failed");
     Readback d2h{st, &r->d2h};
     d2h(r->off, io.f_off, n1 * 8); d2h(r->link_off, link_off, n1 * 8); d2h(r->link_vs, link_vs, NL * 4); d2h(r->link_rel, link_rel, NL);
-    d2h(r->link_roff, link_roff, (NL + 1) * 8); d2h(r->link_toff, link_toff, NL * 8); d2h(r->t_row, g->pt_row.p, TR * 16); d2h(r->t_rel, g->pt_rel.p, TR * 2);
+    d2h(r->link_roff, link_roff, (NL + 1) * 8); d2h(r->link_toff, link_toff, NL * 8); d2h(r->t_row, P.t_row.p, TR * 16); d2h(r->t_rel, P.t_rel.p, TR * 2);
     if (d2h.err == cudaSuccess) d2h.err = cudaStreamSynchronize(st);
     if (d2h.err != cudaSuccess) return fail(ABB_ERR_CUDA, "paths D2H failed: %s", cudaGetErrorString(d2h.err));
     r->rows = r->off.as<int64_t>()[nf];
@@ -1734,17 +1758,17 @@ static int paths_rank(abb_graph *g, const int32_t *findings, int64_t n_findings,
     cudaStream_t st = g->stream;
     const int64_t nf = n_findings, n = g->v.n;
     const bool focused = node_focus != nullptr;
-    if (int rc = g->p_findings.ensure(static_cast<size_t>(nf + 1) * 4)) return rc;
-    if (int rc = g->p_off.ensure(static_cast<size_t>(nf + 1) * 8)) return rc;
+    if (int rc = g->paths.findings.ensure(static_cast<size_t>(nf + 1) * 4)) return rc;
+    if (int rc = g->paths.f_off.ensure(static_cast<size_t>(nf + 1) * 8)) return rc;
     DevBuf d_base, d_tab, d_ncu, d_ntu, d_focus;
-    if (nf) CUDA_TRY(cudaMemcpyAsync(g->p_findings.p, findings, static_cast<size_t>(nf) * 4, cudaMemcpyHostToDevice, st));
+    if (nf) CUDA_TRY(cudaMemcpyAsync(g->paths.findings.p, findings, static_cast<size_t>(nf) * 4, cudaMemcpyHostToDevice, st));
     if (int rc = d_base.upload(base_id, static_cast<size_t>(nf) * 4, st, 4)) return rc;
     if (int rc = d_tab.upload(risk_rank, static_cast<size_t>(n_base) * 75 * 4, st)) return rc;
     if (int rc = d_ncu.upload(ncu, static_cast<size_t>(n) * 4, st, 4)) return rc;
     if (int rc = d_ntu.upload(ntu, static_cast<size_t>(n) * 4, st, 4)) return rc;
     if (focused) { if (int rc = d_focus.upload(node_focus, static_cast<size_t>(n), st, 1)) return rc; }
     abb_paths_io io{};
-    io.n_findings = nf; io.findings = g->p_findings.as<int32_t>(); io.f_off = g->p_off.as<int64_t>();
+    io.n_findings = nf; io.findings = g->paths.findings.as<int32_t>(); io.f_off = g->paths.f_off.as<int64_t>();
     if (int rc = enqueue_paths_count(g, &io, st)) return rc;
     int64_t R = 0;
     CUDA_TRY(cudaMemcpyAsync(&R, io.f_off + nf, 8, cudaMemcpyDeviceToHost, st));
@@ -1761,10 +1785,10 @@ static int paths_rank(abb_graph *g, const int32_t *findings, int64_t n_findings,
     if (!rc) rc = v1.alloc(static_cast<size_t>(R) * 4);
     if (!rc) rc = v2.alloc(static_cast<size_t>(R) * 4);
     if (rc) return rc;
-    PathsArgs A = g->paths_args;
+    PathsArgs A = g->paths.args;
     RankArgs RA{d_base.as<int32_t>(), d_tab.as<uint32_t>(), d_ncu.as<int32_t>(), d_ntu.as<int32_t>(), k1.as<unsigned long long>(), v1.as<uint32_t>(),
                 d_focus.as<uint8_t>(), need};
-    if ((rc = LAUNCH(rank_keys_kernel, row_grid(g, rank_keys_kernel, g->rank_keys_grid), ROW_THREADS, 0, st, A, RA))) return rc;
+    if ((rc = LAUNCH(rank_keys_kernel, row_grid(g, rank_keys_kernel, g->paths.rank_keys_grid), ROW_THREADS, 0, st, A, RA))) return rc;
     // sort input: every row (k1, v1), or the matched rows compacted into (k2, v2); the sorted pairs land in the other pair
     unsigned long long *key_in = k1.as<unsigned long long>(), *key_out = k2.as<unsigned long long>();
     uint32_t *row_in = v1.as<uint32_t>(), *row_out = v2.as<uint32_t>();
@@ -1841,6 +1865,9 @@ extern "C" int abb_exposure_host(abb_graph *g, const int32_t *findings, int64_t 
     // The exposure-path pipeline does not depend on the walk: it runs on its own stream, driven by a helper thread (sizing its
     // factorised result synchronises that stream twice), while this thread stages and runs the walk.  The walk's node arena streams to the host over PCIe
     // as it is produced (zero-copy); the path pipeline's kernels and its factorised result copy fit inside that window.
+    // Both threads use g under the one lock held here, so the two halves must touch disjoint state.  The path half (paths_run and
+    // what it calls) uses only g->v, g->sm_count, g->device, g->paths_stream, g->paths and g->exposure; the walk half uses the walk's
+    // workspaces (g->tiers, g->dedup, g->staging, g->chunked) and never g->paths, g->exposure or g->context.
     abb_paths_result *pr = nullptr;
     int prc = ABB_OK;
     std::string perr;
@@ -1856,7 +1883,7 @@ extern "C" int abb_exposure_host(abb_graph *g, const int32_t *findings, int64_t 
     int rc = chunked_applies(g, &spec, nullptr, nullptr, n_findings) ? walk_host_chunked(g, &spec, findings, n_findings, &wr) : ABB_RETRY_UNCHUNKED;
     auto t1 = now();
     if (rc == ABB_RETRY_UNCHUNKED) {
-        g->last_host_chunks = 1;
+        g->chunked.last_host_chunks = 1;
         rc = walk_device_stage(g, &spec, findings, nullptr, nullptr, n_findings, &io, totals, &h2d, &direct);
         t1 = now();
         if (!rc) rc = walk_collect(g, &spec, io, totals, h2d, &wr, true, &direct);
@@ -1910,49 +1937,51 @@ extern "C" int abb_finding_context_host(abb_graph *g, int32_t max_depth, const i
     DeviceGuard dg(g->device);
     std::lock_guard<std::mutex> lk(g->mu);
     cudaStream_t st = g->stream, cs = g->paths_stream;
+    ContextWorkspace &cx = g->context;
+    DevBuf &scan_tmp = g->paths.scan_tmp;   // the path pipeline's scan scratch: it runs on paths_stream too, never during this call
     const int64_t nq = n_findings;
     const size_t q = static_cast<size_t>(nq), q1 = q + 1;
     auto drain = [&]() { cudaStreamSynchronize(st); cudaStreamSynchronize(cs); };
     int rc = ABB_OK;
-    ENS(d_roots, q1 * 4); ENS(cx_bcnt, q1 * CTX_BUCKETS * 4); ENS(cx_cnt, q1 * 8); ENS(cx_start, q1 * 8);
+    ENS(g->staging.roots, q1 * 4); ENS(cx.bcnt, q1 * CTX_BUCKETS * 4); ENS(cx.cnt, q1 * 8); ENS(cx.start, q1 * 8);
     if (rc) return rc;
     std::unique_ptr<abb_finding_context_result> r(new abb_finding_context_result());
     r->nq = nq;
-    if (nq) CUDA_TRY(cudaMemcpyAsync(g->d_roots.p, findings, q * 4, cudaMemcpyHostToDevice, st));
+    if (nq) CUDA_TRY(cudaMemcpyAsync(g->staging.roots.p, findings, q * 4, cudaMemcpyHostToDevice, st));
     r->h2d = nq * 4;
-    CUDA_TRY(cudaEventRecord(g->cx_staged, st));
-    CUDA_TRY(cudaStreamWaitEvent(cs, g->cx_staged, 0));
+    CUDA_TRY(cudaEventRecord(cx.staged, st));
+    CUDA_TRY(cudaStreamWaitEvent(cs, cx.staged, 0));
     // count pass + scan, next to the walk
     CtxArgs A{};
-    A.g = g->v; A.findings = g->d_roots.as<int32_t>(); A.n = nq;
-    A.bcnt = g->cx_bcnt.as<int32_t>(); A.cnt = g->cx_cnt.as<int64_t>(); A.start = g->cx_start.as<int64_t>();
+    A.g = g->v; A.findings = g->staging.roots.as<int32_t>(); A.n = nq;
+    A.bcnt = cx.bcnt.as<int32_t>(); A.cnt = cx.cnt.as<int64_t>(); A.start = cx.start.as<int64_t>();
     const unsigned grid = warp_grid(g, (nq + 31) / 32);
-    CUDA_TRY(cudaEventRecord(g->cx_ev[0], cs));
+    CUDA_TRY(cudaEventRecord(cx.ev[0], cs));
     CUDA_TRY(cudaMemsetAsync(A.cnt, 0, q1 * 8, cs));
     if (nq) if ((rc = LAUNCH(context_kernel<false>, grid, 256, 0, cs, A))) { drain(); return rc; }
-    if ((rc = scan_i64(g->p_scan_tmp, A.cnt, g->cx_start.as<int64_t>(), nq + 1, cs))) { drain(); return rc; }
-    CUDA_TRY(cudaEventRecord(g->cx_ev[1], cs));
+    if ((rc = scan_i64(scan_tmp, A.cnt, cx.start.as<int64_t>(), nq + 1, cs))) { drain(); return rc; }
+    CUDA_TRY(cudaEventRecord(cx.ev[1], cs));
     // the impact walk, unchanged, into the device arena
     const abb_walk_spec spec = abb_spec_impact_of(max_depth);
     abb_walk_io io{}; unsigned long long totals[3] = {0, 0, 0}; int64_t wh2d = 0;
-    g->last_host_chunks = 1;
+    g->chunked.last_host_chunks = 1;
     if ((rc = walk_device_stage(g, &spec, findings, nullptr, nullptr, nq, &io, totals, &wh2d, nullptr, true))) { drain(); return rc; }
     int64_t total = 0;
-    CUDA_TRY(cudaMemcpyAsync(&total, g->cx_start.as<int64_t>() + nq, 8, cudaMemcpyDeviceToHost, cs));
+    CUDA_TRY(cudaMemcpyAsync(&total, cx.start.as<int64_t>() + nq, 8, cudaMemcpyDeviceToHost, cs));
     CUDA_TRY(cudaStreamSynchronize(cs));
     r->total = total;
-    ENS(cx_src, (total + 1) * 4);
+    ENS(cx.src, (total + 1) * 4);
     if (rc) { drain(); return rc; }
     if (!(r->start.alloc(q * 8) && r->bcnt.alloc(q * CTX_BUCKETS * 4) && r->src.alloc(static_cast<size_t>(total) * 4))) {
         drain(); return fail(ABB_ERR_NOMEM, "pinned host allocation failed");
     }
     // fill pass and its copies on paths_stream, the walk's per-finding arrays on the main stream
-    A.src = g->cx_src.as<int32_t>();
-    CUDA_TRY(cudaEventRecord(g->cx_ev[2], cs));
+    A.src = cx.src.as<int32_t>();
+    CUDA_TRY(cudaEventRecord(cx.ev[2], cs));
     if (nq) if ((rc = LAUNCH(context_kernel<true>, grid, 256, 0, cs, A))) { drain(); return rc; }
-    CUDA_TRY(cudaEventRecord(g->cx_ev[3], cs));
+    CUDA_TRY(cudaEventRecord(cx.ev[3], cs));
     Readback d2h{cs, &r->d2h, cudaGetLastError()};
-    d2h(r->start, g->cx_start.p, q * 8); d2h(r->bcnt, g->cx_bcnt.p, q * CTX_BUCKETS * 4); d2h(r->src, g->cx_src.p, static_cast<size_t>(total) * 4);
+    d2h(r->start, cx.start.p, q * 8); d2h(r->bcnt, cx.bcnt.p, q * CTX_BUCKETS * 4); d2h(r->src, cx.src.p, static_cast<size_t>(total) * 4);
     cudaError_t e = d2h.err;
     if (e != cudaSuccess) { drain(); return fail(ABB_ERR_CUDA, "finding context failed: %s", cudaGetErrorString(e)); }
     abb_walk_result *walk = nullptr;
@@ -1961,8 +1990,8 @@ extern "C" int abb_finding_context_host(abb_graph *g, int32_t max_depth, const i
     if ((e = cudaStreamSynchronize(cs)) != cudaSuccess) { drain(); return fail(ABB_ERR_CUDA, "finding context failed: %s", cudaGetErrorString(e)); }
     r->d2h += r->walk->d2h;
     float a = 0.f, b = 0.f;
-    if (cudaEventElapsedTime(&a, g->ev[0], g->ev[1]) == cudaSuccess) r->walk_ms = a;
-    if (cudaEventElapsedTime(&a, g->cx_ev[0], g->cx_ev[1]) == cudaSuccess && cudaEventElapsedTime(&b, g->cx_ev[2], g->cx_ev[3]) == cudaSuccess) r->context_ms = a + b;
+    if (cudaEventElapsedTime(&a, g->staging.ev_start, g->staging.ev_end) == cudaSuccess) r->walk_ms = a;
+    if (cudaEventElapsedTime(&a, cx.ev[0], cx.ev[1]) == cudaSuccess && cudaEventElapsedTime(&b, cx.ev[2], cx.ev[3]) == cudaSuccess) r->context_ms = a + b;
     *out = r.release();
     return ABB_OK;
 }
@@ -1980,9 +2009,7 @@ extern "C" int abb_finding_context_host(abb_graph *g, int32_t max_depth, const i
 #include "lifecycle_host.inl"
 #include "hops_host.inl"
 
-// Runs with the graph's device current (abb_graph_free); the DevBuf members and the snapshot tables free themselves after it.
+// Runs with the graph's device current (abb_graph_free); the workspaces' events and buffers and the tables free themselves after it.
 abb_graph::~abb_graph() {
     for (cudaStream_t s : {stream, copy_stream, paths_stream}) if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); }
-    for (cudaEvent_t e : {ev_copy, ev_chunk_walked, ev_chunk_copied[0], ev_chunk_copied[1], ev[0], ev[1], ev[2], ev[3], cx_staged, cx_ev[0], cx_ev[1], cx_ev[2], cx_ev[3]})
-        if (e) cudaEventDestroy(e);
 }
